@@ -1,15 +1,16 @@
 #!/usr/bin/env python
-"""bench.py — the BASELINE.json workloads on B200, one JSON line per run.
+"""bench.py — the BASELINE.json workloads on the H100, one JSON line per run.
 
     python bench.py --gpus 1 --steps 10 --warmup 3                 # cfg2 (default): PnP-PGD iterations/s, MRI 256x256 + DRUNet
     python bench.py --impl reference --steps 2 --warmup 1          # the reference's CPU path (oracle port) on the host cores
     torchrun --nproc-per-node N bench.py --gpus N ...              # one rank per GPU, batch sharded (weak scaling)
     python bench.py --config cfg3|cfg4|cfg5 ...                    # the other BASELINE.json workloads (see CONFIGS)
     python bench.py --scaling strong --gpus N                      # cfg2 with the GLOBAL batch of 64 split over N ranks
+    python bench.py ... --dump-outputs DIR                         # also write the timed path's last-step result as DIR/<name>.npy
 
 cfg2 (the configuration the metric is quoted on): one "step" = one PnP-PGD iteration over the whole batch — fused L2 data
 step z = x - gamma (A^T A x - A^T y), then x = DRUNet(z, sigma) — through the package's public optimiser API
-(deepinv_b200.optim.PGD.single_iteration).  The denoiser runs at precision="tc32h" (3 x FP16 split operands on tcgen05:
+(deepinv_b200.optim.PGD.single_iteration).  The denoiser runs at precision="tc32h" (3 x FP16 split operands on wgmma:
 22-bit operands, fp32-grade: whole-network error < 1e-5 against the fp32 reference; "tc32" = the TF32 variant); the line also carries the error of the TIMED
 configuration's K-iteration result against the fp32 CUDA-core path and against the oracle (`parity`), the throughput of the
 fp32 CUDA-core path (`value_fp32`) and of the bf16 tensor-core path with ITS error (`bf16`), per-operator roofline
@@ -54,7 +55,35 @@ def measured_peaks():
         d = json.loads(p.read_text())
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d["bf16_tflops"], "bf16_tflops_sustained": d["bf16_tflops_sustained"],
                 "source": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
+    # H100 SXM data sheet (HBM3 bandwidth, dense BF16): an upper bound, not a measured rate
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "source": "fallback (H100 SXM data sheet)"}
+
+
+DUMP_BYTES = 64 << 20  # --dump-outputs writes at most this much
+
+
+def dump_outputs(out_dir: str, arrays: dict) -> None:
+    """Write what the timed path computed in its last step as <out_dir>/<name>.npy (float32 / float64), so that two builds
+    can be compared output for output on identical inputs.  If the arrays exceed DUMP_BYTES together, each one is replaced
+    by a fixed, seeded sample of its flattened elements (<name>_sample.npy) and the sampled indices (<name>_index.npy)."""
+    import numpy as np
+
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    host = {}
+    for name, t in arrays.items():
+        t = t.detach()
+        t = t.double() if t.dtype == torch.float64 else t.float()
+        host[name] = t.cpu()
+    total = sum(t.numel() * t.element_size() for t in host.values())
+    for name, t in host.items():
+        if total <= DUMP_BYTES:
+            np.save(d / f"{name}.npy", t.numpy())
+            continue
+        k = min(t.numel(), DUMP_BYTES // (2 * len(host) * max(t.element_size(), 8)))
+        idx = torch.randperm(t.numel(), generator=torch.Generator().manual_seed(0))[:k].sort().values
+        np.save(d / f"{name}_sample.npy", t.reshape(-1)[idx].numpy())
+        np.save(d / f"{name}_index.npy", idx.numpy())
 
 
 def cartesian_mask(batch: int, h: int, w: int, accel: int, seed: int) -> torch.Tensor:
@@ -275,7 +304,7 @@ def run_reference(args):
 
 
 # ---------------------------------------------------------------------------------------------
-# B200 arm helpers
+# GPU arm helpers
 # ---------------------------------------------------------------------------------------------
 def time_cuda(fn, iters: int, warmup: int = 3) -> float:
     """average milliseconds per call, CUDA events on the current stream"""
@@ -523,6 +552,8 @@ def run_cfg2(args, world, rank, dev, peaks):
             torch.cuda.profiler.stop()
         ms_total = e0.elapsed_time(e1)
         x_hat = x_hat.clone()
+        if rank == 0 and args.dump_outputs:
+            dump_outputs(args.dump_outputs, {"x_hat": x_hat})
         launches = lib.dinvk_launch_count() - launches0
         if graphed is not None:
             launches = graphed.launches_per_step * args.steps
@@ -691,12 +722,6 @@ def run_cfg2(args, world, rank, dev, peaks):
             C = 64
             gflop_k = 2.0 * BATCH * H * W * C * 9 * C / 1e9
             traffic = None
-            tp = ROOT / "profiles" / "top_kernel_traffic.json"
-            if tp.exists():
-                tj = json.loads(tp.read_text())
-                traffic = tj.get(args.precision, {}).get("dram_bytes_per_launch") if isinstance(tj.get(args.precision), dict) else None
-                if traffic is None and args.precision == "bf16":
-                    traffic = tj.get("dram_bytes_per_launch")
             if args.precision in ("tc32", "tc32h"):
                 from deepinv_b200.models.tc_engine import _pack3x3_slab_tc32
 
@@ -710,10 +735,10 @@ def run_cfg2(args, world, rank, dev, peaks):
                 tf32_peak = peaks["bf16_tflops"] / (1 if fmt else 2)
                 roof = binding_roofline(
                     f"conv_tc32_slab_kernel<{'FmtF16' if fmt else 'FmtTF32'}>: 3x3 conv 64->64, 64x256x256, 3 x "
-                    f"{'FP16' if fmt else 'TF32'} -> fp32 (TMEM + register drain), + residual",
+                    f"{'FP16' if fmt else 'TF32'} -> fp32 (register accumulators + drain), + residual",
                     ms_k, gflop_k, bytes_k, peaks["hbm_gbs"], tf32_peak, traffic,
-                    peaks["source"] + (": HBM copy rate; tensor = bf16 burst (kind::f16 runs at the bf16 rate)" if fmt else
-                                       ": HBM copy rate; tensor = bf16 burst / 2 (dense tf32 rate of the same pipe)"), executed_factor=3.0)
+                    peaks["source"] + (": HBM rate; tensor = bf16 rate (fp16 wgmma runs at the bf16 rate)" if fmt else
+                                       ": HBM rate; tensor = bf16 rate / 2 (dense tf32 rate of the same pipe)"), executed_factor=3.0)
                 del xa, ra, wa
             elif args.precision == "bf16":
                 xa = torch.randn(BATCH, H, W, C, device=dev).to(torch.bfloat16)
@@ -721,9 +746,9 @@ def run_cfg2(args, world, rank, dev, peaks):
                 wa = (torch.randn(C, 9 * C, device=dev) / (3 * C ** 0.5)).to(torch.bfloat16)
                 ms_k = time_cuda(lambda: dops.conv3x3_bf16(xa, wa, res=ra), 20, warmup=3)
                 bytes_k = 3 * BATCH * H * W * C * 2 + C * 9 * C * 2
-                roof = binding_roofline("conv_tc_halo_kernel<64,...>: 3x3 conv 64->64, 64x256x256, bf16 -> fp32 TMEM, +residual", ms_k, gflop_k,
+                roof = binding_roofline("conv_tc_halo_kernel<64,...>: 3x3 conv 64->64, 64x256x256, bf16 -> fp32, +residual", ms_k, gflop_k,
                                         bytes_k, peaks["hbm_gbs"], peaks["bf16_tflops"], traffic,
-                                        peaks["source"] + ": HBM copy rate; tensor = bf16 burst (kernel timed alone)")
+                                        peaks["source"] + ": HBM rate; tensor = bf16 rate (kernel timed alone)")
                 del xa, ra, wa
             else:
                 roof = {"bound": "tensor", "kernel": "DRUNet convolutions (fp32 CUDA-core path, whole forward)", "achieved": tflops,
@@ -788,7 +813,7 @@ def run_cfg2(args, world, rank, dev, peaks):
             "dtype": dtype, "data": "synthetic",
             "config": bench_config("cfg2", world, args.scaling),
             "details": {"denoiser_precision": args.precision, "cuda_graph": graphed is not None, "images_per_gpu": BATCH,
-                        "l2_policy": "per-step working set (>= 1 GB of activations) exceeds the 126 MB L2; no explicit flush"},
+                        "l2_policy": "per-step working set (>= 1 GB of activations) exceeds the 50 MB L2; no explicit flush"},
             "e2e": {"value": (images_per_step / c["batch"]) * 1000.0 / ms_e2e, "unit": c["unit"], "h2d_bytes_per_step": h2d,
                     "d2h_bytes_per_step": d2h, "steps": n_e2e, "mode": e2e_mode},
             "gpu_launches": int(launches),
@@ -908,6 +933,8 @@ def run_other(args, world, rank, dev, peaks):
 
         n0 = lib.dinvk_launch_count()
         ms_step, out, win = timed_steps(step, args.steps, args.warmup, dev, world)
+        if rank == 0 and args.dump_outputs:
+            dump_outputs(args.dump_outputs, {"x_hat": out})
         launches = lib.dinvk_launch_count() - n0 - (0)
         launches = int(launches * args.steps / (args.steps + 0))
         ms_e2e = dist_max(time_cuda(e2e, max(2, min(args.steps, 5)), warmup=1), dev, world)
@@ -967,6 +994,8 @@ def main():
     ap.add_argument("--no-graph", action="store_true", help="time the eager Python loop instead of CUDA-graph replays")
     ap.add_argument("--verify-shards", action="store_true", help="strong scaling: compare the gathered result with rank 0 computing the whole batch")
     ap.add_argument("--lean", action="store_true", help="skip the rank-0 extras (parity, other precisions, rooflines, operators, CPU baseline)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the result of the last one as DIR/<name>.npy (float32, <= 64 MB in all)")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

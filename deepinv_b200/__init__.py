@@ -1,4 +1,4 @@
-"""deepinv_b200 — B200-native (sm_100a) drop-in for DeepInverse's physics-operator hot path.
+"""deepinv_b200 — H100-native (sm_90a) drop-in for DeepInverse's physics-operator hot path.
 
 Public surface mirrors `deepinv`: `deepinv_b200.physics`, `.optim`, `.models`, `.sampling`,
 `.unfolded`.  All arithmetic runs in libdinvk.so (hand-written CUDA behind the C ABI in

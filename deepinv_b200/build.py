@@ -1,6 +1,6 @@
-"""Build libdinvk.so (the sm_100a kernel library) in-tree with nvcc.
+"""Build libdinvk.so (the sm_90a kernel library) in-tree with nvcc.
 
-The shared object is git-ignored but travels to the GPU box with the gpurun snapshot.
+The shared object is a build product (git-ignored).
 `python -m deepinv_b200.build` rebuilds it; `__graft_entry__.build()` calls `build()`.
 """
 from __future__ import annotations
@@ -20,24 +20,12 @@ STAMP = PKG / ".libdinvk.stamp"
 NVCC_FLAGS = [
     "-O3",
     "-std=c++17",
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo",
     "--use_fast_math=false",
     "-Xcompiler", "-fPIC",
     "-shared",
 ]
-
-
-def _cutlass_include() -> list[str]:
-    """CuTe/CUTLASS header tree vendored in site-packages (used by the tcgen05 kernels only)."""
-    import site
-
-    for sp in site.getsitepackages():
-        for rel in ("flashinfer/data/cutlass/include", "tilelang/3rdparty/cutlass/include"):
-            p = Path(sp) / rel
-            if (p / "cute" / "arch" / "mma_sm100_desc.hpp").exists():
-                return ["-I", str(p)]
-    return []
 
 
 def sources() -> list[Path]:
@@ -59,7 +47,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
     flags = [f for f in NVCC_FLAGS if f != "--use_fast_math=false"]
     tmp = LIB.with_suffix(".so.tmp")  # link to a scratch name, then rename: a reader never sees a half-written library
-    cmd = [nvcc, *flags, "-I", str(ROOT / "include"), *_cutlass_include(), "-o", str(tmp), *map(str, sources())]
+    cmd = [nvcc, *flags, "-I", str(ROOT / "include"), "-o", str(tmp), *map(str, sources())]
     if verbose:
         cmd.insert(1, "-Xptxas")
         cmd.insert(2, "-v")

@@ -1,4 +1,4 @@
-// common.cuh — shared infrastructure for libdinvk (sm_100a).
+// common.cuh — shared infrastructure for libdinvk (sm_90a).
 //
 // Two build modes:
 //   * nvcc (the product): real CUDA kernels launched on the caller's stream.
@@ -88,33 +88,13 @@ __host__ __device__ __forceinline__ float2 cmul(float2 a, float2 b) {
 __host__ __device__ __forceinline__ float2 cmul_conj(float2 a, float2 b) {  // a * conj(b)
   return make_float2(a.x * b.x + a.y * b.y, a.y * b.x - a.x * b.y);
 }
-// complex add / sub: on sm_100 one packed FADD2 (add.rn.f32x2) instead of two FADDs — the FFT butterflies are
-// add-dominated, so this removes ~20 % of their instructions; results are bit-identical to the scalar form
-__host__ __device__ __forceinline__ float2 cadd(float2 a, float2 b) {
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ >= 1000) && !defined(DINVK_EMUL)
-  float2 r;
-  asm("{.reg .b64 ra, rb, rc; mov.b64 ra, {%2,%3}; mov.b64 rb, {%4,%5}; add.rn.f32x2 rc, ra, rb; mov.b64 {%0,%1}, rc;}"
-      : "=f"(r.x), "=f"(r.y) : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y));
-  return r;
-#else
-  return make_float2(a.x + b.x, a.y + b.y);
-#endif
-}
-__host__ __device__ __forceinline__ float2 csub(float2 a, float2 b) {
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ >= 1000) && !defined(DINVK_EMUL)
-  float2 r;
-  asm("{.reg .b64 ra, rb, rc; mov.b64 ra, {%2,%3}; mov.b64 rb, {%4,%5}; sub.rn.f32x2 rc, ra, rb; mov.b64 {%0,%1}, rc;}"
-      : "=f"(r.x), "=f"(r.y) : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y));
-  return r;
-#else
-  return make_float2(a.x - b.x, a.y - b.y);
-#endif
-}
+__host__ __device__ __forceinline__ float2 cadd(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }
+__host__ __device__ __forceinline__ float2 csub(float2 a, float2 b) { return make_float2(a.x - b.x, a.y - b.y); }
 __host__ __device__ __forceinline__ float2 cconj(float2 a) { return make_float2(a.x, -a.y); }
 
 inline int ceil_div(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
 
-// number of SMs the grids are sized against (B200: 148); queried once on the real device
+// number of SMs the grids are sized against (H100 SXM: 132); queried once on the real device
 int sm_count();
 
 }  // namespace dinvk

@@ -3,7 +3,7 @@
 // Replaces the ATen calls behind deepinv/models/drunet.py:200-210,323-433 (3x3 conv, ResBlock,
 // strided 2x2 down-conv, transposed 2x2 up-conv, all bias-free) and deepinv/models/dncnn.py:116-131
 // (3x3 conv + bias + ReLU).  This is the parity path (matches the fp32 reference to ~1e-6); the
-// throughput path is the tcgen05 implicit GEMM in conv_tc.cu.
+// throughput path is the wgmma implicit GEMM in conv_tc.cu.
 //
 //   kind 0: 3x3, stride 1, zero padding 1 — register-tiled direct convolution: a CTA computes an
 //           8x32 pixel x 32 output-channel tile, staging 8 input channels (with halo) and their

@@ -1,4 +1,4 @@
-// conv_tc.cu — bf16 tensor-core convolutions for the denoisers: tcgen05 implicit GEMM fed by TMA.
+// conv_tc.cu — bf16 tensor-core convolutions for the denoisers: wgmma implicit GEMM fed by TMA.
 //
 // Replaces the cuDNN/ATen calls behind deepinv/models/drunet.py:200-210 and dncnn.py:116-131 on the
 // throughput path (fp32 parity path: conv_simt.cu).  Activations are NHWC bf16, weights (Cout, taps*Cin)
@@ -7,15 +7,14 @@
 // through a 4-D TMA box shifted by (dx, dy); out-of-range coordinates are zero-filled by TMA, which IS the
 // zero padding of the convolution.
 //
-// Kernel structure (one persistent CTA per SM, 192 threads):
-//   warp 0   : TMA producer — per (tap, 64-channel block): one 4-D box (64 ch x 16 x x 8 y) of activations
-//              = 128 pixels x 128 B, and one 2-D box (64 k x BN rows) of weights, 128-byte swizzled,
-//              into an mbarrier-guarded ring of shared-memory stages.
-//   warp 1   : MMA issuer — one elected thread issues 4 x tcgen05.mma (M=128, N=BN, K=16) per stage into a
-//              TMEM accumulator (fp32), commits the stage back to the producer; two accumulator buffers
-//              in TMEM so that the epilogue of tile i overlaps the main loop of tile i+1.
-//   warps 2-5: epilogue — tcgen05.ld (32 lanes x 32 columns per warp), + residual(s), ReLU, bf16 pack,
-//              128-bit stores (NHWC), or fp32 NCHW stores for the network tail.
+// Kernel structure (one persistent CTA per SM):
+//   warpgroups 0-1: consumers — warpgroup g issues wgmma (M=64, N=BN, K=16) for GEMM rows [64g, 64g+64) of the
+//                   128-pixel tile, accumulates in registers (fp32) and runs the epilogue from its registers:
+//                   + residual(s), ReLU, bf16 pack, NHWC stores, or fp32 NCHW stores for the network tail.
+//   last warp     : TMA producer — per (tap, 64-channel block): one 4-D box (64 ch x 16 x x 8 y) of activations
+//                   = 128 pixels x 128 B, and one 2-D box (64 k x BN rows) of weights, 128-byte swizzled,
+//                   into an mbarrier-guarded ring of shared-memory stages.  While the consumers run an epilogue the
+//                   producer already fills the ring for the next tile.
 #include "common.cuh"
 #include "tc_ptx.cuh"
 
@@ -29,7 +28,8 @@ using bf16 = __nv_bfloat16;
 constexpr int TC_TX = 16, TC_TY = 8;            // pixel tile: 16 x 8 = 128 GEMM rows
 constexpr int TC_KB = 64;                        // K block: 64 bf16 = 128 B = one swizzle row
 constexpr int TC_A_BYTES = 128 * TC_KB * 2;      // 16 KB
-constexpr int TC_THREADS = 320;  // warp 0 TMA, warp 1 MMA, warps 2-5 and 6-9: two epilogue groups (one per TMEM accumulator)
+constexpr int TC_WG_ROWS = 64 * 128 >> 4;        // descriptor offset of GEMM row 64 (64 rows of 128 B, in 16-byte units)
+constexpr int TC_THREADS = 2 * 128 + 32;         // two consumer warpgroups + the TMA producer warp
 
 struct TcMaps {
   CUtensorMap a[4];  // activation views (3x3 and transposed-up: one; strided 2x2 down: one per tap)
@@ -56,10 +56,70 @@ template <int BN>
 struct TcCfg {
   static constexpr int B_BYTES = BN * TC_KB * 2;
   static constexpr int STAGE_BYTES = TC_A_BYTES + B_BYTES;
-  static constexpr int STAGES = (BN >= 256) ? 4 : (BN >= 128 ? 6 : 8);
+  static constexpr int STAGES = BN >= 128 ? 6 : 8;
   static constexpr int SMEM = STAGES * STAGE_BYTES + 1024;  // + alignment slack
-  static constexpr uint32_t TMEM_COLS = (2 * BN <= 32) ? 32 : (2 * BN <= 64 ? 64 : (2 * BN <= 128 ? 128 : (2 * BN <= 256 ? 256 : 512)));
+  static_assert(SMEM <= 227 * 1024, "shared memory budget");
 };
+
+template <int BN>
+__device__ __forceinline__ void mma_bf16(float* d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi, uint32_t accumulate) {
+  if constexpr (BN == 16) tc::wgmma_bf16_n16(d, a_lo, a_hi, b_lo, b_hi, accumulate);
+  else if constexpr (BN == 64) tc::wgmma_bf16_n64(d, a_lo, a_hi, b_lo, b_hi, accumulate);
+  else tc::wgmma_bf16_n128(d, a_lo, a_hi, b_lo, b_hi, accumulate);
+}
+
+// one warp's share of a consumed pipeline stage: the stage's `empty` barrier counts one arrival per consumer warp
+__device__ __forceinline__ void release_stage(uint64_t* bar) {
+  __syncwarp();
+  if ((threadIdx.x & 31) == 0) tc::mbar_arrive(bar);
+}
+
+__device__ __forceinline__ void named_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
+
+// epilogue of one m64 x BN accumulator fragment (see tc_ptx.cuh for the register layout): the caller maps the thread's two
+// rows to pixels (y[r], x[r]); n0 = first GEMM column of the N tile
+template <int BN>
+__device__ __forceinline__ void epilogue_bf16(const ConvTcParams& P, const float* acc, int b, const int (&y)[2], const int (&x)[2], int n0) {
+  const int q = threadIdx.x & 3;
+  const int ncols = P.mode == 2 ? 4 * P.Cout : P.Cout;
+  if (n0 >= ncols) return;
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    if (!(y[r] < P.H && x[r] < P.W)) continue;
+    const long long pix = ((long long)b * P.H + y[r]) * P.W + x[r];
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      const int n = n0 + 8 * j + 2 * q;
+      float v0 = acc[4 * j + 2 * r], v1 = acc[4 * j + 2 * r + 1];
+      if (P.bias) {
+        v0 += (n < P.Cout) ? __ldg(P.bias + n) : 0.f;
+        v1 += (n + 1 < P.Cout) ? __ldg(P.bias + n + 1) : 0.f;
+      }
+      if (P.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+      if (P.out_f32) {
+        // network tail: fp32 NCHW, only the real channels
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          if (n + e < P.Cout) {
+            const long long o = (((long long)b * P.Cout + n + e) * P.H + y[r]) * P.W + x[r];
+            float val = e ? v1 : v0;
+            if (P.add_f32) val += __ldg(P.add_f32 + o);
+            P.out_f32[o] = val;
+          }
+        }
+      } else {
+        long long o = pix * P.Cout + n;
+        if (P.mode == 2) {  // transposed 2x2 stride-2: this N tile belongs to one (dy,dx) tap
+          const int tap = n0 / P.Cout;
+          o = (((long long)b * (2 * P.H) + 2 * y[r] + (tap >> 1)) * (2LL * P.W) + 2 * x[r] + (tap & 1)) * P.Cout + (n - tap * P.Cout);
+        }
+        if (P.res) { const float2 f = __bfloat1622float2(__ldg(reinterpret_cast<const __nv_bfloat162*>(P.res + o))); v0 += f.x; v1 += f.y; }
+        if (P.res2) { const float2 f = __bfloat1622float2(__ldg(reinterpret_cast<const __nv_bfloat162*>(P.res2 + o))); v0 += f.x; v1 += f.y; }
+        *reinterpret_cast<__nv_bfloat162*>(P.out + o) = __floats2bfloat162_rn(v0, v1);
+      }
+    }
+  }
+}
 
 template <int BN>
 __global__ void __launch_bounds__(TC_THREADS, 1)
@@ -69,29 +129,21 @@ conv_tc_kernel(const __grid_constant__ TcMaps M, const ConvTcParams P) {
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
   __shared__ __align__(8) uint64_t full_bar[Cfg::STAGES];
   __shared__ __align__(8) uint64_t empty_bar[Cfg::STAGES];
-  __shared__ __align__(8) uint64_t tfull_bar[2];
-  __shared__ __align__(8) uint64_t tempty_bar[2];
-  __shared__ uint32_t tmem_base_smem;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int pixel_tiles = P.B * P.tiles_y * P.tiles_x;
   const int total_tiles = pixel_tiles * P.n_tiles;
   const int nk = P.ntaps * P.kc_per_tap;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tc::prefetch_tmap(&M.a[0]);
     tc::prefetch_tmap(&M.b);
-    for (int s = 0; s < Cfg::STAGES; ++s) { tc::mbar_init(&full_bar[s], 1); tc::mbar_init(&empty_bar[s], 1); }
-    for (int a = 0; a < 2; ++a) { tc::mbar_init(&tfull_bar[a], 1); tc::mbar_init(&tempty_bar[a], 4); }
+    for (int s = 0; s < Cfg::STAGES; ++s) { tc::mbar_init(&full_bar[s], 1); tc::mbar_init(&empty_bar[s], 8); }
     tc::fence_barrier_init();
   }
-  if (warp == 2) tc::tmem_alloc<Cfg::TMEM_COLS>(&tmem_base_smem);
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ===================== TMA producer =====================
     if (lane == 0) {
       int s = 0; uint32_t ph = 0;
@@ -111,168 +163,64 @@ conv_tc_kernel(const __grid_constant__ TcMaps M, const ConvTcParams P) {
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    // The whole warp runs this loop converged so that every operand stays in uniform registers; one elected lane
-    // issues the tcgen05 instructions.  Per MMA the issue cost is one 32-bit add on the descriptor's low word (the
-    // first version rebuilt 64-bit descriptors in a divergent single-lane branch: ~40 instructions and several
-    // R2UR moves per MMA, which capped the tensor pipe at 24 % / 47 % / 75 % for N = 64 / 128 / 256).
-    constexpr uint32_t idesc = tc::make_idesc_bf16(128, BN);
+  } else {
+    // ===================== consumers: wgmma main loop + epilogue =====================
+    // The group of stage kb is committed before the group of stage kb - 1 is waited for, so the tensor core always has
+    // the next 4 MMAs queued; a stage goes back to the producer once the group that read it has completed.
+    const int wg = warp >> 2;
     constexpr uint32_t HI = tc::desc_hi_sw128(1024);
     const uint32_t smem_lo = tc::smem_u32(smem) >> 4;
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
     int s = 0; uint32_t ph = 0;
-    int acc = 0; uint32_t pa = 0;
     for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
-      tc::mbar_wait(&tempty_bar[acc], pa ^ 1);
-      tc::tc_fence_after();
-      const uint32_t d_tmem = tmem_base + static_cast<uint32_t>(acc * BN);
-      for (int kb = 0; kb < nk; ++kb) {
-        tc::mbar_wait(&full_bar[s], ph);
-        tc::tc_fence_after();
-        const uint32_t a_lo = smem_lo + static_cast<uint32_t>(s) * (Cfg::STAGE_BYTES >> 4);
-        const uint32_t b_lo = a_lo + (TC_A_BYTES >> 4);
-        if (tc::elect_one()) {
-          tc::umma_bf16_lohi(d_tmem, a_lo, HI, b_lo, HI, idesc, kb != 0 ? 1u : 0u);
-          tc::umma_bf16_lohi(d_tmem, a_lo + 2, HI, b_lo + 2, HI, idesc, 1u);
-          tc::umma_bf16_lohi(d_tmem, a_lo + 4, HI, b_lo + 4, HI, idesc, 1u);
-          tc::umma_bf16_lohi(d_tmem, a_lo + 6, HI, b_lo + 6, HI, idesc, 1u);
-          tc::umma_commit(&empty_bar[s]);  // frees the stage once these MMAs have read it
-        }
-        __syncwarp();
-        if (++s == Cfg::STAGES) { s = 0; ph ^= 1; }
-      }
-      if (tc::elect_one()) tc::umma_commit(&tfull_bar[acc]);  // accumulator complete
-      __syncwarp();
-      if (++acc == 2) { acc = 0; pa ^= 1; }
-    }
-  } else {
-    // ===================== epilogue (4 warps, TMEM lane quarter = warp % 4) =====================
-    // two epilogue groups of four warps: group g drains accumulator buffer g, i.e. every other tile, so two tiles'
-    // epilogues (TMEM reads, residual loads, stores) are in flight while the MMA warp fills the next buffer
-    const int q = warp & 3;
-    const int group = (warp - 2) >> 2;
-    const int acc = group;
-    uint32_t pa = 0;
-    int local = 0;
-    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++local) {
-      if ((local & 1) != group) continue;
       const int nt = t / pixel_tiles, pt = t - nt * pixel_tiles;
       const int b = pt / (P.tiles_y * P.tiles_x), r = pt - b * (P.tiles_y * P.tiles_x);
       const int y0 = (r / P.tiles_x) * TC_TY, x0 = (r % P.tiles_x) * TC_TX;
-      const int m = q * 32 + lane;
-      const int y = y0 + m / TC_TX, x = x0 + m % TC_TX;
-      const bool inside = (y < P.H) && (x < P.W);
-      tc::mbar_wait(&tfull_bar[acc], pa);
-      tc::tc_fence_after();
-      const uint32_t t_addr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>(acc * BN);
-      constexpr int CH = (BN >= 32) ? 32 : 16;
-#pragma unroll 1
-      for (int c0 = 0; c0 < BN; c0 += CH) {
-        float v[CH];
-        if constexpr (CH == 32) {
-          uint32_t rr[32];
-          tc::tmem_ld_32x32b_x32(t_addr + c0, rr);
-          tc::tmem_ld_wait();
+      int pend = -1;
+      for (int kb = 0; kb < nk; ++kb) {
+        tc::mbar_wait(&full_bar[s], ph);
+        const uint32_t a_lo = smem_lo + static_cast<uint32_t>(s) * (Cfg::STAGE_BYTES >> 4) + wg * TC_WG_ROWS;
+        const uint32_t b_lo = smem_lo + static_cast<uint32_t>(s) * (Cfg::STAGE_BYTES >> 4) + (TC_A_BYTES >> 4);
+        tc::wgmma_fence();
 #pragma unroll
-          for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(rr[i]);
-        } else {
-          uint32_t rr[16];
-          tc::tmem_ld_32x32b_x16(t_addr + c0, rr);
-          tc::tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(rr[i]);
-        }
-        const int n0 = nt * BN + c0;
-        const int ncols = P.mode == 2 ? 4 * P.Cout : P.Cout;
-        if (P.bias) {
-#pragma unroll
-          for (int i = 0; i < CH; ++i) v[i] += (n0 + i < P.Cout) ? __ldg(P.bias + n0 + i) : 0.f;
-        }
-        if (inside && n0 < ncols) {
-          const long long pix = ((long long)b * P.H + y) * P.W + x;
-          if (P.out_f32) {
-            // network tail: fp32 NCHW, only the real channels
-#pragma unroll
-            for (int i = 0; i < CH; ++i) {
-              const int c = n0 + i;
-              if (c < P.Cout) {
-                const long long o = (((long long)b * P.Cout + c) * P.H + y) * P.W + x;
-                float val = v[i];
-                if (P.relu) val = fmaxf(val, 0.f);
-                if (P.add_f32) val += __ldg(P.add_f32 + o);
-                P.out_f32[o] = val;
-              }
-            }
-          } else {
-            if (P.relu) {
-#pragma unroll
-              for (int i = 0; i < CH; ++i) v[i] = fmaxf(v[i], 0.f);
-            }
-            long long o = pix * P.Cout + n0;
-            if (P.mode == 2) {  // transposed 2x2 stride-2: this N tile belongs to one (dy,dx) tap
-              const int tap = n0 / P.Cout;
-              o = (((long long)b * (2 * P.H) + 2 * y + (tap >> 1)) * (2LL * P.W) + 2 * x + (tap & 1)) * P.Cout + (n0 - tap * P.Cout);
-            }
-            // 256-bit accesses (CH is 32 here: bf16 outputs use N tiles >= 64): one full 32-byte sector per lane
-            if (P.res) {
-#pragma unroll
-              for (int j = 0; j < CH / 16; ++j) {
-                uint32_t u[8];
-                tc::ldg256(P.res + o + j * 16, u);
-#pragma unroll
-                for (int e = 0; e < 8; ++e) { const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&u[e])); v[j * 16 + 2 * e] += f.x; v[j * 16 + 2 * e + 1] += f.y; }
-              }
-            }
-            if (P.res2) {
-#pragma unroll
-              for (int j = 0; j < CH / 16; ++j) {
-                uint32_t u[8];
-                tc::ldg256(P.res2 + o + j * 16, u);
-#pragma unroll
-                for (int e = 0; e < 8; ++e) { const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&u[e])); v[j * 16 + 2 * e] += f.x; v[j * 16 + 2 * e + 1] += f.y; }
-              }
-            }
-#pragma unroll
-            for (int j = 0; j < CH / 16; ++j) {
-              uint32_t u[8];
-#pragma unroll
-              for (int e = 0; e < 8; ++e) {
-                const __nv_bfloat162 hh = __floats2bfloat162_rn(v[j * 16 + 2 * e], v[j * 16 + 2 * e + 1]);
-                u[e] = *reinterpret_cast<const uint32_t*>(&hh);
-              }
-              tc::stg256(P.out + o + j * 16, u);
-            }
-          }
-        }
+        for (int k = 0; k < 4; ++k) mma_bf16<BN>(acc, a_lo + 2 * k, HI, b_lo + 2 * k, HI, (kb | k) != 0 ? 1u : 0u);
+        tc::wgmma_commit();
+        tc::wgmma_wait<1>();
+        if (pend >= 0) release_stage(&empty_bar[pend]);
+        pend = s;
+        if (++s == Cfg::STAGES) { s = 0; ph ^= 1; }
       }
-      tc::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&tempty_bar[acc]);
-      pa ^= 1;
+      tc::wgmma_wait<0>();
+      tc::reg_fence<BN / 2>(acc);
+      if (pend >= 0) release_stage(&empty_bar[pend]);
+      int y[2], x[2];
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        const int m = 64 * wg + 16 * (warp & 3) + (lane >> 2) + 8 * rr;
+        y[rr] = y0 + m / TC_TX; x[rr] = x0 + m % TC_TX;
+      }
+      epilogue_bf16<BN>(P, acc, b, y, x, nt * BN);
     }
   }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tc::tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
 // 3x3 convolution with HALO REUSE (64- and 128-channel layers).
 //
-// The per-tap kernel above re-reads every activation tile 9 times from L2; ncu shows the 64/128-channel layers are
-// L2-bandwidth bound because of it (lts ~55-58 %, 11-14 TB/s of L2->SM traffic, tensor pipe 24 % / 47 % active).
-// Here one TMA box brings an (18 y) x (16 x) x 64-channel slab (the 16x8 output tile plus its halo; 16 pixels per
-// slab row keeps every 8-row group 1024-byte periodic) into shared memory ONCE per 64-channel block, and the nine
-// taps are nine UMMA descriptors into that same slab: start address shifted by (ky*16 + kx) rows of 128 B,
-// stride between 8-row groups = one slab row (2048 B).  The 128-byte swizzle is a function of the shared-memory
-// ADDRESS bits [7:9] on both the TMA write and the UMMA read, so a start address that is not 1024-byte aligned needs
-// no descriptor base_offset (measured on B200: base_offset = 0 is bit-correct, base_offset = kx is wrong).
-// L2->SM activation traffic drops 4x (36 KB instead of 144 KB per tile and channel block).  For 64->64 layers the
-// whole weight tensor (9 x 64 x 64 bf16 = 72 KB) stays resident in shared memory for the lifetime of the CTA.
+// The per-tap kernel above re-reads every activation tile 9 times from L2.  Here one TMA box brings an (18 y) x (SLAB_X x)
+// x 64-channel slab (the output tile plus its halo; a multiple of 8 positions per slab row keeps every 8-row group
+// 1024-byte periodic) into shared memory ONCE per 64-channel block, and the nine taps are nine wgmma descriptors into that
+// same slab: start address shifted by (ky*SLAB_X + kx) rows of 128 B, stride between 8-row groups = one slab row.  The
+// 128-byte swizzle is a function of the shared-memory ADDRESS bits on both the TMA write and the wgmma read, so a start
+// address that is not 1024-byte aligned needs no descriptor base offset.  L2->SM activation traffic drops about 4x.
+// For 64->64 layers the whole weight tensor (9 x 64 x 64 bf16 = 72 KB) stays resident in shared memory for the lifetime
+// of the CTA.
 // ---------------------------------------------------------------------------------------------------------------
-// MH x-halves per CTA tile: the tile is 8*MH x by 16 y output pixels, half h (x in [8h, 8h+8)) is one M=128 accumulator.
-// MH = 2 shares every weight tile between two MMAs groups (256 pixels per B stage): the streamed-weight layers
-// (>= 128 channels) were bound by the L2->SM weight traffic (TMA round trips), not by the tensor pipe.
+// MH x-halves per CTA tile: the tile is 8*MH x by 16 y output pixels.  Consumer warpgroup g owns the m64 block
+// (x-half g / 2, y-half g % 2): 8 x 8 pixels, GEMM row m = 8 * (y - y-half start) + (x - x-half start).
+// MH = 2 shares every weight tile between four warpgroups (256 pixels per B stage).
 constexpr int HL_TY = 16;
 template <int MH> struct HaloGeom {
   static constexpr int TX = 8 * MH;
@@ -292,15 +240,12 @@ struct HaloCfg {
   static constexpr int SMEM = A_STAGES * G::SLAB_BYTES + B_STAGES * B_TILE + 1024;
   static_assert(SMEM <= 227 * 1024, "shared memory budget");
   static_assert(G::SLAB_BYTES % 1024 == 0, "slab stages must stay 1024-byte aligned");
-  static constexpr int NSETS = (2 * MH * BN <= 512) ? 2 : 1;   // accumulator sets (one set = MH accumulators of BN columns)
-  static_assert(MH * BN <= 512, "tensor memory budget");
-  static_assert(MH == 2 || NSETS == 2, "one-half tiles need two accumulator sets (one per epilogue group)");
-  static constexpr int ACC_COLS = NSETS * MH * BN;
-  static constexpr uint32_t TMEM_COLS = ACC_COLS <= 32 ? 32 : (ACC_COLS <= 64 ? 64 : (ACC_COLS <= 128 ? 128 : (ACC_COLS <= 256 ? 256 : 512)));
+  static constexpr int NWG = 2 * MH;                 // consumer warpgroups
+  static constexpr int THREADS = 128 * NWG + 32;     // + the TMA producer warp
 };
 
 template <int BN, bool RESIDENT, int AST, int BST, int MH>
-__global__ void __launch_bounds__(TC_THREADS, 1)
+__global__ void __launch_bounds__((HaloCfg<BN, RESIDENT, AST, BST, MH>::THREADS), 1)
 conv_tc_halo_kernel(const __grid_constant__ TcMaps M, const ConvTcParams P) {
   using Cfg = HaloCfg<BN, RESIDENT, AST, BST, MH>;
   using G = HaloGeom<MH>;
@@ -311,30 +256,22 @@ conv_tc_halo_kernel(const __grid_constant__ TcMaps M, const ConvTcParams P) {
   __shared__ __align__(8) uint64_t aempty[Cfg::A_STAGES];
   __shared__ __align__(8) uint64_t bfull[Cfg::B_STAGES];
   __shared__ __align__(8) uint64_t bempty[Cfg::B_STAGES];
-  __shared__ __align__(8) uint64_t tfull_bar[2];
-  __shared__ __align__(8) uint64_t tempty_bar[2];
-  __shared__ uint32_t tmem_base_smem;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int pixel_tiles = P.B * P.tiles_y * P.tiles_x;
   const int total_tiles = pixel_tiles * P.n_tiles;
   const int nkc = P.kc_per_tap;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tc::prefetch_tmap(&M.a[0]);
     tc::prefetch_tmap(&M.b);
-    for (int s = 0; s < Cfg::A_STAGES; ++s) { tc::mbar_init(&afull[s], 1); tc::mbar_init(&aempty[s], 1); }
-    for (int s = 0; s < Cfg::B_STAGES; ++s) { tc::mbar_init(&bfull[s], 1); tc::mbar_init(&bempty[s], 1); }
-    for (int a = 0; a < 2; ++a) { tc::mbar_init(&tfull_bar[a], 1); tc::mbar_init(&tempty_bar[a], 4 * MH); }
+    for (int s = 0; s < Cfg::A_STAGES; ++s) { tc::mbar_init(&afull[s], 1); tc::mbar_init(&aempty[s], 4 * Cfg::NWG); }
+    for (int s = 0; s < Cfg::B_STAGES; ++s) { tc::mbar_init(&bfull[s], 1); tc::mbar_init(&bempty[s], 4 * Cfg::NWG); }
     tc::fence_barrier_init();
   }
-  if (warp == 2) tc::tmem_alloc<Cfg::TMEM_COLS>(&tmem_base_smem);
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
 
-  if (warp == 0) {
+  if (warp == 4 * Cfg::NWG) {
     if (lane == 0) {
       if (RESIDENT) {  // the whole 3x3 weight tensor, once
         for (int tap = 0; tap < 9; ++tap) {
@@ -364,210 +301,88 @@ conv_tc_halo_kernel(const __grid_constant__ TcMaps M, const ConvTcParams P) {
         }
       }
     }
-  } else if (warp == 1) {
-    // converged warp, uniform operands, one elected issuer (see conv_tc_kernel)
-    constexpr uint32_t idesc = tc::make_idesc_bf16(128, BN);
+  } else {
+    const int wg = warp >> 2;
+    const int half = wg >> 1, yh = wg & 1;
     constexpr uint32_t HI_A = tc::desc_hi_sw128(G::SLAB_X * 128);
     constexpr uint32_t HI_B = tc::desc_hi_sw128(1024);
-    const uint32_t slab_lo0 = tc::smem_u32(smem) >> 4;
+    // this warpgroup's block starts at slab row 8 * yh, position 8 * half (128-byte rows = 8 descriptor units)
+    const uint32_t slab_lo0 = (tc::smem_u32(smem) >> 4) + static_cast<uint32_t>((8 * yh * G::SLAB_X + 8 * half) * 8);
     const uint32_t bt_lo0 = tc::smem_u32(smem_b) >> 4;
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
     int sa = 0; uint32_t pha = 0;
     int sb = 0; uint32_t phb = 0;
-    int set = 0; uint32_t pset = 0;  // bit s of pset: phase of accumulator set s
     if (RESIDENT) {
       for (int tap = 0; tap < 9; ++tap) tc::mbar_wait(&bfull[tap], 0);
     }
     for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
-      tc::mbar_wait(&tempty_bar[set], ((pset >> set) & 1u) ^ 1u);
-      tc::tc_fence_after();
-      const uint32_t d_tmem = tmem_base + static_cast<uint32_t>(set * MH * BN);
+      const int nt = t / pixel_tiles, pt = t - nt * pixel_tiles;
+      const int b = pt / (P.tiles_y * P.tiles_x), r = pt - b * (P.tiles_y * P.tiles_x);
+      const int y0 = (r / P.tiles_x) * HL_TY, x0 = (r % P.tiles_x) * G::TX;
+      int pend_a = -1, pend_b = -1;  // stages read by the previous wgmma group: released once it has completed
       for (int kc = 0; kc < nkc; ++kc) {
         tc::mbar_wait(&afull[sa], pha);
-        tc::tc_fence_after();
         const uint32_t slab_lo = slab_lo0 + static_cast<uint32_t>(sa) * (G::SLAB_BYTES >> 4);
         if (RESIDENT) {
-          if (tc::elect_one()) {
+          tc::wgmma_fence();
 #pragma unroll
-            for (int tap = 0; tap < 9; ++tap) {
-              const uint32_t b_lo = bt_lo0 + static_cast<uint32_t>(tap * (Cfg::B_TILE >> 4));
+          for (int tap = 0; tap < 9; ++tap) {
+            const uint32_t a_lo = slab_lo + static_cast<uint32_t>(((tap / 3) * G::SLAB_X + (tap % 3)) * 8);
+            const uint32_t b_lo = bt_lo0 + static_cast<uint32_t>(tap * (Cfg::B_TILE >> 4));
 #pragma unroll
-              for (int h = 0; h < MH; ++h) {
-                const uint32_t a_lo = slab_lo + static_cast<uint32_t>(((tap / 3) * G::SLAB_X + (tap % 3) + 8 * h) * 8);
-#pragma unroll
-                for (int k = 0; k < 4; ++k)
-                  tc::umma_bf16_lohi(d_tmem + h * BN, a_lo + 2 * k, HI_A, b_lo + 2 * k, HI_B, idesc, (tap | k) != 0 ? 1u : (kc != 0 ? 1u : 0u));
-              }
-            }
-            tc::umma_commit(&aempty[sa]);
+            for (int k = 0; k < 4; ++k) mma_bf16<BN>(acc, a_lo + 2 * k, HI_A, b_lo + 2 * k, HI_B, (kc | tap | k) != 0 ? 1u : 0u);
           }
-          __syncwarp();
+          tc::wgmma_commit();
+          tc::wgmma_wait<1>();
+          if (pend_a >= 0) release_stage(&aempty[pend_a]);
+          pend_a = sa;
         } else {
 #pragma unroll 1
           for (int tap = 0; tap < 9; ++tap) {
             tc::mbar_wait(&bfull[sb], phb);
-            tc::tc_fence_after();
             const uint32_t a_lo = slab_lo + static_cast<uint32_t>(((tap / 3) * G::SLAB_X + (tap % 3)) * 8);
             const uint32_t b_lo = bt_lo0 + static_cast<uint32_t>(sb) * (Cfg::B_TILE >> 4);
-            if (tc::elect_one()) {
+            tc::wgmma_fence();
 #pragma unroll
-              for (int h = 0; h < MH; ++h) {
-                tc::umma_bf16_lohi(d_tmem + h * BN, a_lo + 64 * h, HI_A, b_lo, HI_B, idesc, (kc | tap) != 0 ? 1u : 0u);
-                tc::umma_bf16_lohi(d_tmem + h * BN, a_lo + 64 * h + 2, HI_A, b_lo + 2, HI_B, idesc, 1u);
-                tc::umma_bf16_lohi(d_tmem + h * BN, a_lo + 64 * h + 4, HI_A, b_lo + 4, HI_B, idesc, 1u);
-                tc::umma_bf16_lohi(d_tmem + h * BN, a_lo + 64 * h + 6, HI_A, b_lo + 6, HI_B, idesc, 1u);
-              }
-              tc::umma_commit(&bempty[sb]);
-              if (tap == 8) tc::umma_commit(&aempty[sa]);
-            }
-            __syncwarp();
+            for (int k = 0; k < 4; ++k) mma_bf16<BN>(acc, a_lo + 2 * k, HI_A, b_lo + 2 * k, HI_B, (kc | tap | k) != 0 ? 1u : 0u);
+            tc::wgmma_commit();
+            tc::wgmma_wait<1>();
+            if (pend_b >= 0) release_stage(&bempty[pend_b]);
+            if (pend_a >= 0) release_stage(&aempty[pend_a]);
+            pend_b = sb;
+            pend_a = tap == 8 ? sa : -1;
             if (++sb == Cfg::B_STAGES) { sb = 0; phb ^= 1; }
           }
         }
         if (++sa == Cfg::A_STAGES) { sa = 0; pha ^= 1; }
       }
-      if (tc::elect_one()) tc::umma_commit(&tfull_bar[set]);
-      __syncwarp();
-      pset ^= 1u << set;
-      if (++set == Cfg::NSETS) set = 0;
-    }
-  } else {
-    // two epilogue groups of four warps (TMEM lane quarter = warp % 4).  MH == 1: group g drains accumulator set g,
-    // i.e. every other tile.  MH == 2: both groups work on every tile, group g drains x-half g of the current set.
-    const int q = warp & 3;
-    const int group = (warp - 2) >> 2;
-    const int half = (MH == 2) ? group : 0;
-    uint32_t pset = 0;
-    int local = 0;
-    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++local) {
-      if (MH == 1 && (local & 1) != group) continue;
-      const int set = (MH == 1) ? group : (local % Cfg::NSETS);
-      const uint32_t pa = (pset >> set) & 1u;
-      pset ^= 1u << set;
-      const int nt = t / pixel_tiles, pt = t - nt * pixel_tiles;
-      const int b = pt / (P.tiles_y * P.tiles_x), r = pt - b * (P.tiles_y * P.tiles_x);
-      const int y0 = (r / P.tiles_x) * HL_TY, x0 = (r % P.tiles_x) * G::TX;
-      const int m = q * 32 + lane;
-      const int y = y0 + (m >> 3), x = x0 + 8 * half + (m & 7);
-      const bool inside = (y < P.H) && (x < P.W);
-      const uint32_t t_addr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>((set * MH + half) * BN);
-      if constexpr (BN == 16) {
-      // network tail (Cout <= 16): fp32 NCHW stores of the real channels, optional "+ x" term
-      tc::mbar_wait(&tfull_bar[set], pa);
-      tc::tc_fence_after();
-      uint32_t rr[16];
-      tc::tmem_ld_32x32b_x16(t_addr, rr);
-      tc::tmem_ld_wait();
-      if (inside) {
+      tc::wgmma_wait<0>();
+      tc::reg_fence<BN / 2>(acc);
+      if (pend_b >= 0) release_stage(&bempty[pend_b]);
+      if (pend_a >= 0) release_stage(&aempty[pend_a]);
+      int y[2], x[2];
 #pragma unroll
-        for (int c = 0; c < 16; ++c) {
-          if (c < P.Cout) {
-            const long long o = (((long long)b * P.Cout + c) * P.H + y) * P.W + x;
-            float val = __uint_as_float(rr[c]);
-            if (P.bias) val += __ldg(P.bias + c);
-            if (P.relu) val = fmaxf(val, 0.f);
-            if (P.add_f32) val += __ldg(P.add_f32 + o);
-            P.out_f32[o] = val;
-          }
-        }
+      for (int rr = 0; rr < 2; ++rr) {
+        const int m = 16 * (warp & 3) + (lane >> 2) + 8 * rr;
+        y[rr] = y0 + 8 * yh + (m >> 3); x[rr] = x0 + 8 * half + (m & 7);
       }
-      } else {
-      // residual operands are fetched one 32-channel chunk AHEAD of the accumulator reads, starting before the
-      // accumulator is even complete: their HBM latency overlaps the MMA main loop instead of serialising the epilogue
-      const long long obase = (((long long)b * P.H + y) * P.W + x) * P.Cout + (long long)nt * BN;
-      uint4 ra[4], rb[4];
-      auto fetch = [&](int c0, uint4 (&a)[4], uint4 (&bb)[4]) {  // 2 x 256-bit loads per residual: a full sector per lane
-        if (inside && P.res) {
-          uint32_t t0[8], t1[8];
-          tc::ldg256(P.res + obase + c0, t0);
-          tc::ldg256(P.res + obase + c0 + 16, t1);
-          a[0] = make_uint4(t0[0], t0[1], t0[2], t0[3]); a[1] = make_uint4(t0[4], t0[5], t0[6], t0[7]);
-          a[2] = make_uint4(t1[0], t1[1], t1[2], t1[3]); a[3] = make_uint4(t1[4], t1[5], t1[6], t1[7]);
-        }
-        if (inside && P.res2) {
-          uint32_t t0[8], t1[8];
-          tc::ldg256(P.res2 + obase + c0, t0);
-          tc::ldg256(P.res2 + obase + c0 + 16, t1);
-          bb[0] = make_uint4(t0[0], t0[1], t0[2], t0[3]); bb[1] = make_uint4(t0[4], t0[5], t0[6], t0[7]);
-          bb[2] = make_uint4(t1[0], t1[1], t1[2], t1[3]); bb[3] = make_uint4(t1[4], t1[5], t1[6], t1[7]);
-        }
-      };
-      fetch(0, ra, rb);
-      tc::mbar_wait(&tfull_bar[set], pa);
-      tc::tc_fence_after();
-#pragma unroll 1
-      for (int c0 = 0; c0 < BN; c0 += 32) {
-        float v[32];
-        uint32_t rr[32];
-        tc::tmem_ld_32x32b_x32(t_addr + c0, rr);
-        uint4 na[4], nb[4];
-        if (c0 + 32 < BN) fetch(c0 + 32, na, nb);
-        tc::tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(rr[i]);
-        const int n0 = nt * BN + c0;
-        if (P.bias) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) v[i] += __ldg(P.bias + n0 + i);
-        }
-        if (inside) {
-          if (P.relu) {
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] = fmaxf(v[i], 0.f);
-          }
-          if (P.res) {
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&ra[j]);
-#pragma unroll
-              for (int e = 0; e < 4; ++e) { const float2 f = __bfloat1622float2(h[e]); v[j * 8 + 2 * e] += f.x; v[j * 8 + 2 * e + 1] += f.y; }
-            }
-          }
-          if (P.res2) {
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&rb[j]);
-#pragma unroll
-              for (int e = 0; e < 4; ++e) { const float2 f = __bfloat1622float2(h[e]); v[j * 8 + 2 * e] += f.x; v[j * 8 + 2 * e + 1] += f.y; }
-            }
-          }
-#pragma unroll
-          for (int j = 0; j < 2; ++j) {  // 2 x 256-bit stores: 16 channels each
-            uint32_t u[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) {
-              const __nv_bfloat162 hh = __floats2bfloat162_rn(v[j * 16 + 2 * e], v[j * 16 + 2 * e + 1]);
-              u[e] = *reinterpret_cast<const uint32_t*>(&hh);
-            }
-            tc::stg256(P.out + obase + c0 + j * 16, u);
-          }
-        }
-        if (c0 + 32 < BN) {
-#pragma unroll
-          for (int j = 0; j < 4; ++j) { ra[j] = na[j]; rb[j] = nb[j]; }
-        }
-      }
-      }
-      tc::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&tempty_bar[set]);
+      epilogue_bf16<BN>(P, acc, b, y, x, nt * BN);
     }
   }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tc::tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
 // Network HEAD: 3x3 convolution from a few-channel NCHW fp32 image (+ optional constant noise-level channel, DRUNet's
-// sigma map) to 64 NHWC bf16 channels.  Going through the generic kernel means padding 3 channels to 64 (a 537 MB
-// converter write and 9 taps x 64 channels of zeros through L2 and the tensor pipe): 640 us per DRUNet forward.
+// sigma map) to 64 NHWC bf16 channels.  Going through the generic kernel means padding 3 channels to 64 (a large
+// converter write and 9 taps x 64 channels of zeros through L2 and the tensor pipe).
 // Here the im2col row of a pixel (K = 9 taps x CT channels <= 64, k = tap*CT + c) is BUILT IN SHARED MEMORY by CUDA
-// threads straight from the fp32 input (33 MB), in the 128-byte-swizzled K-major layout the UMMA descriptor expects
+// threads straight from the fp32 input, in the 128-byte-swizzled K-major layout the wgmma descriptor expects
 // (16-byte chunk j of row m lives at chunk j ^ (m & 7)), so the whole layer is one K=64 GEMM step per 128-pixel tile
-// and the only real traffic is the 537 MB output write.
-//   warps 0-7 : two builder groups (tile parity g -> A stage g), 128 threads each, one pixel per thread
-//   warp  8   : MMA issuer (4 x tcgen05.mma M128 N64 K16 per tile)
-//   warps 9-16: two epilogue groups (accumulator g), TMEM lane quarter = warp % 4
+// and the only real traffic is the output write.
+//   warpgroup g (of 2) owns every other tile: its 128 threads build the tile's 128 rows (one pixel each) in A stage g,
+//   issue 2 x 4 wgmma (M=64, N=64, K=16) and store the two m64 accumulators.
 // ---------------------------------------------------------------------------------------------------------------
 struct HeadParams {
   const float* x;          // (B, C, H, W) fp32
@@ -582,7 +397,7 @@ struct HeadParams {
   int tiles_x, tiles_y;
 };
 constexpr int HD_TX = 32, HD_TY = 4;
-constexpr int HD_THREADS = 17 * 32;
+constexpr int HD_THREADS = 2 * 128;
 constexpr int HD_SMEM = 2 * TC_A_BYTES + 64 * 128 + 1024;
 
 template <int CT>
@@ -593,22 +408,10 @@ __global__ void __launch_bounds__(HD_THREADS, 1) conv_head_kernel(const HeadPara
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
   uint8_t* smem_b = smem + 2 * TC_A_BYTES;
-  __shared__ __align__(8) uint64_t afull[2];
-  __shared__ __align__(8) uint64_t aempty[2];
-  __shared__ __align__(8) uint64_t tfull_bar[2];
-  __shared__ __align__(8) uint64_t tempty_bar[2];
-  __shared__ uint32_t tmem_base_smem;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int total_tiles = P.B * P.tiles_y * P.tiles_x;
 
-  if (threadIdx.x == 0) {
-    for (int a = 0; a < 2; ++a) {
-      tc::mbar_init(&afull[a], 128); tc::mbar_init(&aempty[a], 1);
-      tc::mbar_init(&tfull_bar[a], 1); tc::mbar_init(&tempty_bar[a], 4);
-    }
-    tc::fence_barrier_init();
-  }
   // zero both A stages once (chunks >= NCH are never written again), stage the weights with the same swizzle
   for (int i = threadIdx.x; i < 2 * TC_A_BYTES / 16; i += HD_THREADS) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
   for (int i = threadIdx.x; i < 64 * 8; i += HD_THREADS) {
@@ -617,146 +420,95 @@ __global__ void __launch_bounds__(HD_THREADS, 1) conv_head_kernel(const HeadPara
     *reinterpret_cast<uint4*>(smem_b + n * 128 + ((j ^ (n & 7)) << 4)) = v;
   }
   tc::fence_proxy_async();
-  if (warp == 8) tc::tmem_alloc<128>(&tmem_base_smem);
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
 
-  if (warp < 8) {
-    // ===================== builders =====================
-    // The 9*CT input values of a pixel are fetched with UNCONDITIONAL loads from clamped coordinates (then masked), one
-    // tile ahead of their use: all loads of a tile are independent and in flight while the previous tile is converted,
-    // stored and handed to the MMA warp (the first version interleaved predicated loads with their uses and spent
-    // ~3400 cycles per tile waiting on them, ncu: 73 % long-scoreboard stalls).
-    const int group = warp >> 2;
-    const int m = (warp & 3) * 32 + lane;  // GEMM row = (warp&3) tile row, lane = x
-    uint8_t* row = smem + group * TC_A_BYTES + m * 128;
-    const int tiles_per_img = P.tiles_y * P.tiles_x;
-    auto gather = [&](int t, float (&v)[9 * CT]) {
-      const int b = t / tiles_per_img, r = t - b * tiles_per_img;
-      const int y = (r / P.tiles_x) * HD_TY + (warp & 3), x = (r % P.tiles_x) * HD_TX + lane;
-      const float fillv = P.has_fill ? (P.fill_batch ? __ldg(P.fill_batch + b) : P.fill_scalar) : 0.f;
-      const float* img = P.x + (long long)b * P.C * P.H * P.W;
+  // The 9*CT input values of a pixel are fetched with UNCONDITIONAL loads from clamped coordinates (then masked), one
+  // tile ahead of their use: all loads of a tile are independent and in flight while the previous tile is converted,
+  // stored and multiplied.
+  const int group = warp >> 2;
+  const int m = (warp & 3) * 32 + lane;  // GEMM row = (warp&3) tile row, lane = x
+  uint8_t* row = smem + group * TC_A_BYTES + m * 128;
+  const int tiles_per_img = P.tiles_y * P.tiles_x;
+  auto gather = [&](int t, float (&v)[9 * CT]) {
+    const int b = t / tiles_per_img, r = t - b * tiles_per_img;
+    const int y = (r / P.tiles_x) * HD_TY + (warp & 3), x = (r % P.tiles_x) * HD_TX + lane;
+    const float fillv = P.has_fill ? (P.fill_batch ? __ldg(P.fill_batch + b) : P.fill_scalar) : 0.f;
+    const float* img = P.x + (long long)b * P.C * P.H * P.W;
 #pragma unroll
-      for (int tap = 0; tap < 9; ++tap) {
-        const int yy = y + tap / 3 - 1, xx = x + tap % 3 - 1;
-        const bool inb = (yy >= 0) && (yy < P.H) && (xx >= 0) && (xx < P.W);
-        const int yc = min(max(yy, 0), P.H - 1), xc = min(max(xx, 0), P.W - 1);
+    for (int tap = 0; tap < 9; ++tap) {
+      const int yy = y + tap / 3 - 1, xx = x + tap % 3 - 1;
+      const bool inb = (yy >= 0) && (yy < P.H) && (xx >= 0) && (xx < P.W);
+      const int yc = min(max(yy, 0), P.H - 1), xc = min(max(xx, 0), P.W - 1);
 #pragma unroll
-        for (int c = 0; c < CT; ++c) {
-          const int cc = min(c, P.C - 1);
-          const float val = __ldg(img + ((long long)cc * P.H + yc) * P.W + xc);
-          v[tap * CT + c] = inb ? ((c < P.C) ? val : fillv) : 0.f;  // a select, not a branch: the load above is unconditional
-        }
-      }
-    };
-    uint32_t ph = 0;
-    const int stride2 = 2 * gridDim.x;
-    int t = blockIdx.x + group * gridDim.x;
-    float cur[9 * CT];
-    if (t < total_tiles) gather(t, cur);
-    for (; t < total_tiles; t += stride2) {
-      float nxt[9 * CT];
-      const bool more = t + stride2 < total_tiles;
-      if (more) gather(t + stride2, nxt);
-      tc::mbar_wait(&aempty[group], ph ^ 1);
-#pragma unroll
-      for (int j = 0; j < NCH; ++j) {
-        uint4 u;
-        __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&u);
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int k0 = j * 8 + 2 * e;
-          h[e] = __floats2bfloat162_rn(k0 < KREAL ? cur[k0] : 0.f, k0 + 1 < KREAL ? cur[k0 + 1] : 0.f);
-        }
-        *reinterpret_cast<uint4*>(row + ((j ^ (m & 7)) << 4)) = u;
-      }
-      tc::fence_proxy_async();  // generic-proxy writes -> visible to the tensor core's async-proxy reads
-      tc::mbar_arrive(&afull[group]);
-      ph ^= 1;
-      if (more) {
-#pragma unroll
-        for (int k = 0; k < 9 * CT; ++k) cur[k] = nxt[k];
+      for (int c = 0; c < CT; ++c) {
+        const int cc = min(c, P.C - 1);
+        const float val = __ldg(img + ((long long)cc * P.H + yc) * P.W + xc);
+        v[tap * CT + c] = inb ? ((c < P.C) ? val : fillv) : 0.f;  // a select, not a branch: the load above is unconditional
       }
     }
-  } else if (warp == 8) {
-    // ===================== MMA issuer =====================
-    constexpr uint32_t idesc = tc::make_idesc_bf16(128, 64);
-    constexpr uint32_t HI = tc::desc_hi_sw128(1024);
-    const uint32_t a_lo0 = tc::smem_u32(smem) >> 4;
-    const uint32_t b_lo = tc::smem_u32(smem_b) >> 4;
-    uint32_t ph[2] = {0, 0};
-    int local = 0;
-    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++local) {
-      const int g = local & 1;
-      tc::mbar_wait(&tempty_bar[g], ph[g] ^ 1);
-      tc::mbar_wait(&afull[g], ph[g]);
-      tc::tc_fence_after();
-      const uint32_t d_tmem = tmem_base + static_cast<uint32_t>(g * 64);
-      const uint32_t a_lo = a_lo0 + static_cast<uint32_t>(g) * (TC_A_BYTES >> 4);
-      if (tc::elect_one()) {
+  };
+  constexpr uint32_t HI = tc::desc_hi_sw128(1024);
+  const uint32_t a_lo = (tc::smem_u32(smem) >> 4) + static_cast<uint32_t>(group) * (TC_A_BYTES >> 4);
+  const uint32_t b_lo = tc::smem_u32(smem_b) >> 4;
+  float acc[2][32];
 #pragma unroll
-        for (int k = 0; k < 4; ++k) tc::umma_bf16_lohi(d_tmem, a_lo + 2 * k, HI, b_lo + 2 * k, HI, idesc, k != 0 ? 1u : 0u);
-        tc::umma_commit(&aempty[g]);
-        tc::umma_commit(&tfull_bar[g]);
+  for (int i = 0; i < 32; ++i) { acc[0][i] = 0.f; acc[1][i] = 0.f; }
+  const int stride2 = 2 * gridDim.x;
+  int t = blockIdx.x + group * gridDim.x;
+  float cur[9 * CT];
+  if (t < total_tiles) gather(t, cur);
+  for (; t < total_tiles; t += stride2) {
+    float nxt[9 * CT];
+    const bool more = t + stride2 < total_tiles;
+    if (more) gather(t + stride2, nxt);
+#pragma unroll
+    for (int j = 0; j < NCH; ++j) {
+      uint4 u;
+      __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&u);
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int k0 = j * 8 + 2 * e;
+        h[e] = __floats2bfloat162_rn(k0 < KREAL ? cur[k0] : 0.f, k0 + 1 < KREAL ? cur[k0 + 1] : 0.f);
       }
-      __syncwarp();
-      ph[g] ^= 1;
+      *reinterpret_cast<uint4*>(row + ((j ^ (m & 7)) << 4)) = u;
     }
-  } else {
-    // ===================== epilogue =====================
-    const int q = warp & 3;
-    const int group = (warp - 9) >> 2;
-    uint32_t pa = 0;
-    int local = 0;
-    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++local) {
-      if ((local & 1) != group) continue;
-      const int b = t / (P.tiles_y * P.tiles_x), r = t - b * (P.tiles_y * P.tiles_x);
-      const int y = (r / P.tiles_x) * HD_TY + q, x = (r % P.tiles_x) * HD_TX + lane;
-      const bool inside = (y < P.H) && (x < P.W);
-      bf16* o = P.out + (((long long)b * P.H + y) * P.W + x) * 64;
-      tc::mbar_wait(&tfull_bar[group], pa);
-      tc::tc_fence_after();
-      const uint32_t t_addr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>(group * 64);
+    tc::fence_proxy_async();  // generic-proxy writes -> visible to the tensor core's async-proxy reads
+    named_sync(1 + group, 128);
+    tc::wgmma_fence();
 #pragma unroll
-      for (int c0 = 0; c0 < 64; c0 += 32) {
-        uint32_t rr[32];
-        tc::tmem_ld_32x32b_x32(t_addr + c0, rr);
-        tc::tmem_ld_wait();
-        float v[32];
+    for (int hh = 0; hh < 2; ++hh)
 #pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(rr[i]);
-        if (P.bias) {
+      for (int k = 0; k < 4; ++k) tc::wgmma_bf16_n64(acc[hh], a_lo + hh * TC_WG_ROWS + 2 * k, HI, b_lo + 2 * k, HI, k != 0 ? 1u : 0u);
+    tc::wgmma_commit();
+    tc::wgmma_wait<0>();
+    tc::reg_fence<32>(acc[0]);
+    tc::reg_fence<32>(acc[1]);
+    named_sync(1 + group, 128);  // every warp's reads of the A stage are complete before it is rewritten
+    const int b = t / tiles_per_img, r = t - b * tiles_per_img;
+    const int y0 = (r / P.tiles_x) * HD_TY, x0 = (r % P.tiles_x) * HD_TX;
+    const int q = lane & 3;
 #pragma unroll
-          for (int i = 0; i < 32; ++i) v[i] += __ldg(P.bias + c0 + i);
-        }
-        if (P.relu) {
+    for (int hh = 0; hh < 2; ++hh)
 #pragma unroll
-          for (int i = 0; i < 32; ++i) v[i] = fmaxf(v[i], 0.f);
-        }
-        if (inside) {
+      for (int rr = 0; rr < 2; ++rr) {
+        const int mm = 64 * hh + 16 * (warp & 3) + (lane >> 2) + 8 * rr;
+        const int y = y0 + mm / HD_TX, x = x0 + mm % HD_TX;
+        if (y >= P.H || x >= P.W) continue;
+        bf16* o = P.out + (((long long)b * P.H + y) * P.W + x) * 64;
 #pragma unroll
-          for (int j = 0; j < 2; ++j) {
-            uint32_t u[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) {
-              const __nv_bfloat162 hh = __floats2bfloat162_rn(v[j * 16 + 2 * e], v[j * 16 + 2 * e + 1]);
-              u[e] = *reinterpret_cast<const uint32_t*>(&hh);
-            }
-            tc::stg256(o + c0 + j * 16, u);
-          }
+        for (int j = 0; j < 8; ++j) {
+          const int c = 8 * j + 2 * q;
+          float v0 = acc[hh][4 * j + 2 * rr], v1 = acc[hh][4 * j + 2 * rr + 1];
+          if (P.bias) { v0 += __ldg(P.bias + c); v1 += __ldg(P.bias + c + 1); }
+          if (P.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+          *reinterpret_cast<__nv_bfloat162*>(o + c) = __floats2bfloat162_rn(v0, v1);
         }
       }
-      tc::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&tempty_bar[group]);
-      pa ^= 1;
+    if (more) {
+#pragma unroll
+      for (int k = 0; k < 9 * CT; ++k) cur[k] = nxt[k];
     }
   }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 8) tc::tmem_dealloc<128>(tmem_base);
 }
 
 // ---- layout converters ---------------------------------------------------------------------------------
@@ -972,13 +724,11 @@ static int launch_conv_halo(TcMaps& M, ConvTcParams& P, const void* x, void* str
   const long long tiles = (long long)P.B * P.tiles_y * P.tiles_x * P.n_tiles;
   const int grid = (int)std::min<long long>(tiles, sm_count());
   count_launch();
-  conv_tc_halo_kernel<BN, RESIDENT, AST, BST, MH><<<grid, TC_THREADS, Cfg::SMEM, (cudaStream_t)stream>>>(M, P);
+  conv_tc_halo_kernel<BN, RESIDENT, AST, BST, MH><<<grid, Cfg::THREADS, Cfg::SMEM, (cudaStream_t)stream>>>(M, P);
   return DINVK_POST_LAUNCH();
 }
 
-// halo mode (DINVK_CONV_HALO): 0 = off (per-tap kernel), 1 = on (default).  The UMMA descriptors into the slab use
-// base_offset 0: the 128-byte swizzle is a function of the shared-memory address, so a start address that is not
-// 1024-byte aligned needs no correction (base_offset = kx was tried on B200 and produces wrong results).
+// halo mode (DINVK_CONV_HALO): 0 = off (per-tap kernel), 1 = on (default).
 static int halo_mode() {
   static int mode = -1;
   if (mode < 0) {
@@ -988,14 +738,14 @@ static int halo_mode() {
   return mode;
 }
 
-static int pick_bn(int rows) { return rows % 256 == 0 ? 256 : (rows % 128 == 0 ? 128 : 64); }
+// N tile: at most 128 columns, so that a consumer warpgroup's m64 accumulator is at most 64 registers per thread
+static int pick_bn(int rows) { return rows % 128 == 0 ? 128 : 64; }
 
 static int dispatch_conv_tc(int bn, const TcMaps& M, const ConvTcParams& P, void* stream) {
   switch (bn) {
     case 16: return launch_conv_tc<16>(M, P, stream);
     case 64: return launch_conv_tc<64>(M, P, stream);
-    case 128: return launch_conv_tc<128>(M, P, stream);
-    default: return launch_conv_tc<256>(M, P, stream);
+    default: return launch_conv_tc<128>(M, P, stream);
   }
 }
 
@@ -1012,13 +762,10 @@ static int conv3x3_tc(const void* x, const void* weight, const float* bias, cons
   int rc;
   // slab + halo kernel (activations read once per 64-channel block instead of once per tap):
   //   64 -> 64 and the 64 -> (<=16) tail with the weights resident in shared memory; >= 128 output channels with streamed
-  //   weights.  Body layers use 16x16-pixel CTA tiles = TWO M=128 accumulators per weight tile (measured on B200 at the
-  //   DRUNet shapes, one vs two accumulators: 64 ch 309 -> 285 us, 128 ch 280 -> 238 us, 256 ch 219 -> 203 us).
-  // DINVK_HALO_VARIANT selects the measured alternatives (1: previous one-accumulator kernels / per-tap kernel for N=256).
-  static const int variant = getenv("DINVK_HALO_VARIANT") ? atoi(getenv("DINVK_HALO_VARIANT")) : 0;
+  //   weights.  64-channel layers use 16x16-pixel CTA tiles (four m64 blocks share every weight tile), the streamed layers
+  //   8x16-pixel tiles (two m64 blocks of up to 64 accumulator registers per thread).
   const bool halo_tail = out_f32 && Cin == 64 && rows == 16 && !getenv("DINVK_NO_HALO_TAIL");
-  // (Cin >= 512 at 32x32 pixels: 512 tile jobs over 148 CTAs quantise badly with 256-pixel tiles; the per-tap kernel is faster)
-  const bool halo_body = !out_f32 && ((rows == 64 && Cin == 64) || bn == 128 || (bn == 256 && Cin < 512 && variant != 1));
+  const bool halo_body = !out_f32 && ((rows == 64 && Cin == 64) || bn == 128);
   if (halo_mode() != 0 && (halo_tail || halo_body)) {
     if ((rc = make_w_map(&M.b, weight, 9 * Cin, rows, bn))) return rc;
     ConvTcParams P;
@@ -1029,19 +776,8 @@ static int conv3x3_tc(const void* x, const void* weight, const float* bias, cons
     P.tiles_x = 0; P.tiles_y = 0; P.n_tiles = rows / bn;  // tiles_x/y: set by the launcher from the kernel's tile geometry
     P.relu = act; P.res = (const bf16*)res; P.res2 = (const bf16*)res2; P.out = (bf16*)out; P.out_f32 = out_f32; P.add_f32 = add_f32; P.bias = bias;
     if (halo_tail) return launch_conv_halo<16, true, 4, 0, 1>(M, P, x, stream);
-    if (bn == 64) {
-      switch (variant) {
-        case 1: return launch_conv_halo<64, true, 4, 0, 1>(M, P, x, stream);
-        default: return launch_conv_halo<64, true, 2, 0, 2>(M, P, x, stream);
-      }
-    }
-    if (bn == 128) {
-      switch (variant) {
-        case 1: return launch_conv_halo<128, false, 2, 8, 1>(M, P, x, stream);
-        default: return launch_conv_halo<128, false, 2, 7, 2>(M, P, x, stream);
-      }
-    }
-    return launch_conv_halo<256, false, 2, 3, 2>(M, P, x, stream);
+    if (bn == 64) return launch_conv_halo<64, true, 2, 0, 2>(M, P, x, stream);
+    return launch_conv_halo<128, false, 2, 8, 1>(M, P, x, stream);
   }
   if ((rc = make_act_map(&M.a[0], x, B, H, W, Cin, (long long)Cin * 2, (long long)W * Cin * 2, (long long)H * W * Cin * 2))) return rc;
   M.a[1] = M.a[0]; M.a[2] = M.a[0]; M.a[3] = M.a[0];

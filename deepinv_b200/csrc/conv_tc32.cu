@@ -1,25 +1,27 @@
-// conv_tc32.cu — fp32-grade tensor-core convolutions for the denoisers: split-operand (3 x TF32) tcgen05 implicit GEMM.
+// conv_tc32.cu — fp32-grade tensor-core convolutions for the denoisers: split-operand wgmma implicit GEMM.
 //
 // The reference computes DRUNet / DnCNN in fp32 (deepinv/models/drunet.py:200-263, dncnn.py:121-140).  The bf16 path
-// (conv_tc.cu) is fast but 3e-2 away from it; the CUDA-core path (conv_simt.cu) matches it but runs at 2 % of the tensor
-// peak.  Here every fp32 value v is carried as the pair  hi = tf32(v) (cvt.rna), lo = v - hi (exact), and a product
-// sum is evaluated as  sum a_hi*b_hi  +  sum (a_hi*b_lo + a_lo*b_hi)  with tcgen05.mma kind::tf32 (fp32 accumulate in
-// TMEM): the dropped a_lo*b_lo term is 2^-22 relative.  The two sums live in separate TMEM column ranges ("main" and
-// "corr"), and the accumulators are DRAINED into fp32 registers every `win` pipeline stages (round-to-nearest adds on the
-// CUDA cores) so that the tensor core's accumulator rounding never sees more than a short partial sum.
+// (conv_tc.cu) is fast but 3e-2 away from it; the CUDA-core path (conv_simt.cu) matches it but runs at a small fraction of
+// the tensor peak.  Here every fp32 value v is carried as a pair (hi, lo) with hi + lo == v, and a product sum is evaluated
+// as  sum a_hi*b_hi  +  sum (a_hi*b_lo + a_lo*b_hi)  on the tensor cores (fp32 accumulate): the dropped a_lo*b_lo term is
+// 2^-22 relative.  The two sums live in separate accumulator columns ("main" and "corr"), and the accumulators are DRAINED
+// into separate fp32 registers every `win` pipeline stages (round-to-nearest adds on the CUDA cores) so that the tensor
+// core's accumulator rounding never sees more than a short partial sum.
 //
 // Activation layout in HBM ("split16"): NHWC with channels in blocks of 16, hi and lo interleaved per block:
 //   x[b][y][x][c/16][p][c%16],  p = 0: hi, 1: lo      (fp32 words; 8 bytes per element; a pixel of a 16-channel block is
-//   one 128-byte row = one swizzle row of the K-major UMMA operand).  hi + lo == v exactly, so residual / skip additions
+//   one 128-byte row = one swizzle row of the K-major wgmma operand).  hi + lo == v exactly, so residual / skip additions
 //   read both words and lose nothing.
 // Weight layout: per 64-row N tile 128 rows [W_hi (64 couts); W_lo (64 couts)], K-major, k = tap*Cin + c, both parts
 //   rounded to tf32.
-// One MMA "k8 step" on a 128-byte A row: steps 0,1 = the 16 hi channels, steps 2,3 = the 16 lo channels.
+// One MMA "k step" on a 128-byte A row: steps 0,1 = the hi channels, steps 2,3 = the lo channels.
 //   hi step: A_hi x [W_hi; W_lo]  (N = 128)  -> columns [0,64) main, [64,128) corr
 //   lo step: A_lo x  W_hi         (N =  64)  -> columns [64,128) corr
+// With wgmma's register accumulators the corr columns of the N = 128 fragment are exactly the registers of an N = 64
+// fragment (registers 32..63), so the lo steps accumulate into the upper half of the same register array.
 //
-// Kernel (persistent, one CTA per SM, 320 threads): warp 0 TMA producer, warp 1 MMA issuer, warps 2-9 drain/epilogue
-// (TMEM lane quarter = warp % 4, column half = (warp - 2) / 4).
+// Kernels (persistent, one CTA per SM): consumer warpgroups issue wgmma (M = 64 rows each), drain and run the epilogue
+// from registers; one extra warp is the TMA producer.
 #include "common.cuh"
 #ifndef DINVK_EMUL
 #include "tc_ptx.cuh"
@@ -41,14 +43,13 @@ inline void stg256(void* p, const uint32_t (&r)[8]) { std::memcpy(p, r, 32); }
 namespace dinvk {
 namespace t32 {
 
-constexpr int TX = 16, TY = 8;             // pixel tile of one accumulator: 16 x 8 = 128 GEMM rows
+constexpr int TX = 16, TY = 8;             // pixel tile of one CTA: 16 x 8 = 128 GEMM rows
 constexpr int A_TILE = 128 * 128;          // one 16-channel block of 128 pixels: 16 KB
 constexpr int B_TILE = 128 * 128;          // [W_hi; W_lo] x 32 channels: 16 KB
 constexpr int STAGE = 2 * A_TILE + B_TILE; // two channel blocks of one tap + their weights
 constexpr int STAGES = 4;
 constexpr int SMEM = STAGES * STAGE + 1024;
-constexpr int THREADS = 320;
-constexpr uint32_t TMEM_COLS = 256;        // 2 accumulator buffers x (64 main + 64 corr)
+constexpr int THREADS = 2 * 128 + 32;      // two consumer warpgroups (GEMM rows [0, 64), [64, 128)) + the TMA producer warp
 
 __device__ __forceinline__ float rna_tf32(float x) {
 #ifndef DINVK_EMUL
@@ -63,9 +64,9 @@ __device__ __forceinline__ float rna_tf32(float x) {
 // ---- the two split formats ------------------------------------------------------------------------------------------
 // A 128-byte row block holds CH channels as [hi CH | lo CH].
 //   FmtTF32 ("split16", fp32 words): hi = tf32(v) (cvt.rna), lo = v - hi (exact; the tensor core truncates it to tf32);
-//            kind::tf32, K = 8 per MMA.  No range restriction.
+//            wgmma .tf32, K = 8 per MMA.  No range restriction.
 //   FmtF16  ("split32h", fp16 words): hi = fp16(v), lo = fp16((v - hi) * 2^11) — the low part is scaled so that it sits in
-//            fp16's normal range; the correction accumulators are weighted 2^-11 in the drain.  kind::f16, K = 16 per MMA: the
+//            fp16's normal range; the correction accumulators are weighted 2^-11 in the drain.  wgmma .f16, K = 16 per MMA: the
 //            same 22-bit operands at TWICE the channels per MMA and half the bytes per element.  Range: |v| < 65504 — an
 //            activation beyond it raises the sticky overflow flag and the network tail answers NaN (loud, never silent).
 struct FmtTF32 {
@@ -74,10 +75,6 @@ struct FmtTF32 {
   static constexpr float CORR = 1.0f;
 #ifndef DINVK_EMUL
   static constexpr CUtensorMapDataType TM = CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
-  // cute::UMMA::InstrDescriptor: c_format F32 (1) at [4,6), a/b_format TF32 (2) at [7,10) / [10,13), K-major, N>>3, M>>4
-  __host__ __device__ static constexpr uint32_t idesc(int M, int N) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | (static_cast<uint32_t>(N >> 3) << 17) | (static_cast<uint32_t>(M >> 4) << 24);
-  }
 #endif
 };
 struct FmtF16 {
@@ -86,42 +83,40 @@ struct FmtF16 {
   static constexpr float CORR = 4.8828125e-4f;  // 2^-11
 #ifndef DINVK_EMUL
   static constexpr CUtensorMapDataType TM = CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-  // a/b_format F16 (0)
-  __host__ __device__ static constexpr uint32_t idesc(int M, int N) {
-    return (1u << 4) | (static_cast<uint32_t>(N >> 3) << 17) | (static_cast<uint32_t>(M >> 4) << 24);
-  }
 #endif
 };
 
 #ifndef DINVK_EMUL
-template <class F>
-__device__ __forceinline__ void umma(uint32_t tmem_d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi, uint32_t idesc,
-                                     uint32_t accumulate) {
+template <class F, int N>
+__device__ __forceinline__ void mma(float* d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi, uint32_t accumulate) {
   if constexpr (F::ID == 0) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        ".reg .b64 da, db;\n\t"
-        "mov.b64 da, {%1, %2};\n\t"
-        "mov.b64 db, {%3, %4};\n\t"
-        "setp.ne.b32 p, %6, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], da, db, %5, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
-        : "memory");
+    if constexpr (N == 128) tc::wgmma_tf32_n128(d, a_lo, a_hi, b_lo, b_hi, accumulate);
+    else tc::wgmma_tf32_n64(d, a_lo, a_hi, b_lo, b_hi, accumulate);
   } else {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        ".reg .b64 da, db;\n\t"
-        "mov.b64 da, {%1, %2};\n\t"
-        "mov.b64 db, {%3, %4};\n\t"
-        "setp.ne.b32 p, %6, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
-        : "memory");
+    if constexpr (N == 128) tc::wgmma_f16_n128(d, a_lo, a_hi, b_lo, b_hi, accumulate);
+    else tc::wgmma_f16_n64(d, a_lo, a_hi, b_lo, b_hi, accumulate);
   }
+}
+// one 128-byte A row block [hi CH | lo CH] (descriptor a) against the weight rows [W_hi; W_lo] at descriptor b (the block's
+// CH channels): acc[0, 32) main += A_hi W_hi, acc[32, 64) corr += A_hi W_lo + A_lo W_hi.  `fresh` = 0 restarts both.
+template <class F>
+__device__ __forceinline__ void mma_block(float* acc, uint32_t a, uint32_t a_hi, uint32_t b, uint32_t b_hi, uint32_t fresh) {
+  mma<F, 128>(acc, a, a_hi, b, b_hi, fresh);             // hi, first half of the block  x [W_hi; W_lo]
+  mma<F, 128>(acc, a + 2, a_hi, b + 2, b_hi, 1u);        // hi, second half
+  mma<F, 64>(acc + 32, a + 4, a_hi, b, b_hi, 1u);        // lo, first half  x W_hi
+  mma<F, 64>(acc + 32, a + 6, a_hi, b + 2, b_hi, 1u);    // lo, second half
+}
+// v[i] (row 16 * (warp % 4) + lane / 4 + 8 * ((i >> 1) & 1), column 8 * (i >> 2) + 2 * (lane % 4) + (i & 1)) += main + corr
+template <class F>
+__device__ __forceinline__ void drain(float* v, const float* acc) {
+#pragma unroll
+  for (int i = 0; i < 32; ++i) v[i] += acc[i] + acc[32 + i] * F::CORR;
+}
+
+// one warp's share of a consumed pipeline stage: the stage's `empty` barrier counts one arrival per consumer warp
+__device__ __forceinline__ void release_stage(uint64_t* bar) {
+  __syncwarp();
+  if ((threadIdx.x & 31) == 0) tc::mbar_arrive(bar);
 }
 
 struct Maps {
@@ -131,7 +126,7 @@ struct Maps {
 
 struct Params {
   int B, H, W, Cin, Cout;   // H, W: the pixel grid the GEMM rows tile (3x3: image; down: OUTPUT grid; up: INPUT grid)
-  int ntaps, kc_per_tap;    // kc_per_tap = Cin / 32 (pipeline stages per tap)
+  int ntaps, kc_per_tap;    // kc_per_tap = Cin / (2 CH) (pipeline stages per tap)
   int dx[9], dy[9], amap[9];
   int mode;                 // 0: same-grid store; 2: 2x up-scatter (GEMM column = tap*Cout + co)
   int tiles_x, tiles_y, n_tiles;
@@ -145,7 +140,6 @@ struct Params {
   int ngrp;                 // work-item order: `ngrp` N tiles (64 output channels each) of a pixel tile are ADJACENT work items, so that
                             // the CTAs that share its activations run at the same time and all but the first read them from L2
                             // (1 = all pixel tiles of N tile 0 first: every activation byte crosses HBM n_tiles times); divides n_tiles
-  int dbg;                  // timing experiments only (DINVK_TC32_DBG): 1 no TMA loads, 2 no epilogue memory traffic, 4 no TMEM drains
 };
 
 // work item t -> (pixel tile, N tile): t = ((nt / g) * pixel_tiles + pt) * g + nt % g, g = P.ngrp
@@ -215,35 +209,88 @@ __device__ __forceinline__ void add_split(const typename F::elem* p, float* v) {
 }
 
 #ifndef DINVK_EMUL
+// the same two conversions for one channel pair (c, c + 1), c even, as the wgmma epilogues hold them; p points at the hi
+// element of channel c in its block (the lo element is CH further)
+template <class F>
+__device__ __forceinline__ void add_split_pair(const typename F::elem* p, float& a, float& b) {
+  if constexpr (F::ID == 0) {
+    const float2 h = __ldg(reinterpret_cast<const float2*>(p)), l = __ldg(reinterpret_cast<const float2*>(p + F::CH));
+    a += h.x + l.x;
+    b += h.y + l.y;
+  } else {
+    const float2 h = __half22float2(__ldg(reinterpret_cast<const __half2*>(p)));
+    const float2 l = __half22float2(__ldg(reinterpret_cast<const __half2*>(p + F::CH)));
+    a += h.x + l.x * F::CORR;
+    b += h.y + l.y * F::CORR;
+  }
+}
+template <class F>
+__device__ __forceinline__ bool store_split_pair(typename F::elem* p, float a, float b) {
+  if constexpr (F::ID == 0) {
+    const float ha = rna_tf32(a), hb = rna_tf32(b);
+    *reinterpret_cast<float2*>(p) = make_float2(ha, hb);
+    *reinterpret_cast<float2*>(p + F::CH) = make_float2(a - ha, b - hb);
+    return false;
+  } else {
+    const __half h0 = __float2half_rn(a), h1 = __float2half_rn(b);
+    const __half l0 = __float2half_rn((a - __half2float(h0)) * 2048.0f), l1 = __float2half_rn((b - __half2float(h1)) * 2048.0f);
+    *reinterpret_cast<__half2*>(p) = __halves2half2(h0, h1);
+    *reinterpret_cast<__half2*>(p + F::CH) = __halves2half2(l0, l1);
+    return !(fabsf(a) < 65000.0f) || !(fabsf(b) < 65000.0f);
+  }
+}
+
+// epilogue of the drained sums v (see drain) of one m64 x 64-column block: bias, ReLU, residuals, split store.  The caller
+// maps the thread's two rows to pixels; n0 = first GEMM column of the N tile.
+template <class F>
+__device__ __forceinline__ void epilogue_split(const Params& P, float* v, int b, const int (&y)[2], const int (&x)[2], int n0) {
+  using E = typename F::elem;
+  const int q = threadIdx.x & 3;
+  const int tap = P.mode == 2 ? n0 / P.Cout : 0;
+  const int c0 = n0 - tap * P.Cout;   // output channel of GEMM column n0
+  bool bad = false;
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    if (!(y[r] < P.H && x[r] < P.W)) continue;
+    long long pix;   // output pixel index
+    if (P.mode == 2) pix = ((long long)b * (2 * P.H) + 2 * y[r] + (tap >> 1)) * (2LL * P.W) + 2 * x[r] + (tap & 1);
+    else pix = ((long long)b * P.H + y[r]) * P.W + x[r];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int c = c0 + 8 * j + 2 * q;
+      float a = v[4 * j + 2 * r], bb = v[4 * j + 2 * r + 1];
+      if (P.bias) { a += __ldg(P.bias + c); bb += __ldg(P.bias + c + 1); }
+      if (P.relu) { a = fmaxf(a, 0.f); bb = fmaxf(bb, 0.f); }
+      const long long o = pix * P.Cout * 2 + (c / F::CH) * 2 * F::CH + (c % F::CH);
+      if (P.res) add_split_pair<F>(static_cast<const E*>(P.res) + o, a, bb);
+      if (P.res2) add_split_pair<F>(static_cast<const E*>(P.res2) + o, a, bb);
+      bad |= store_split_pair<F>(static_cast<E*>(P.out) + o, a, bb);
+    }
+  }
+  if (bad && P.flag) atomicOr(P.flag, 1);
+}
+
 template <class F>
 __global__ void __launch_bounds__(THREADS, 1) conv_tc32_kernel(const __grid_constant__ Maps M, const Params P) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
   __shared__ __align__(8) uint64_t full_bar[STAGES];
   __shared__ __align__(8) uint64_t empty_bar[STAGES];
-  __shared__ __align__(8) uint64_t tfull_bar[2];
-  __shared__ __align__(8) uint64_t tempty_bar[2];
-  __shared__ uint32_t tmem_base_smem;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int pixel_tiles = P.B * P.tiles_y * P.tiles_x;
   const int total_tiles = pixel_tiles * P.n_tiles;
   const int nk = P.ntaps * P.kc_per_tap;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tc::prefetch_tmap(&M.a[0]);
     tc::prefetch_tmap(&M.b);
-    for (int s = 0; s < STAGES; ++s) { tc::mbar_init(&full_bar[s], 1); tc::mbar_init(&empty_bar[s], 1); }
-    for (int a = 0; a < 2; ++a) { tc::mbar_init(&tfull_bar[a], 1); tc::mbar_init(&tempty_bar[a], 8); }
+    for (int s = 0; s < STAGES; ++s) { tc::mbar_init(&full_bar[s], 1); tc::mbar_init(&empty_bar[s], 8); }
     tc::fence_barrier_init();
   }
-  if (warp == 2) tc::tmem_alloc<TMEM_COLS>(&tmem_base_smem);
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ===================== TMA producer =====================
     if (lane == 0) {
       int s = 0; uint32_t ph = 0;
@@ -264,175 +311,113 @@ __global__ void __launch_bounds__(THREADS, 1) conv_tc32_kernel(const __grid_cons
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (converged warp, one elected lane) =====================
-    constexpr uint32_t ID128 = F::idesc(128, 128), ID64 = F::idesc(128, 64);
+  } else {
+    // ===================== consumers: wgmma, drains, epilogue =====================
+    const int wg = warp >> 2;
     constexpr uint32_t HI = tc::desc_hi_sw128(1024);
     const uint32_t smem_lo = tc::smem_u32(smem) >> 4;
-    int s = 0; uint32_t ph = 0;
-    int acc = 0; uint32_t pa = 0;
-    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
-      int in_win = 0;
-      for (int kb = 0; kb < nk; ++kb) {
-        if (in_win == 0) {
-          tc::mbar_wait(&tempty_bar[acc], pa ^ 1);
-          tc::tc_fence_after();
-        }
-        tc::mbar_wait(&full_bar[s], ph);
-        tc::tc_fence_after();
-        const uint32_t d = tmem_base + static_cast<uint32_t>(acc * 128);
-        const uint32_t a0 = smem_lo + static_cast<uint32_t>(s) * (STAGE >> 4);
-        const uint32_t b0 = a0 + (2 * A_TILE >> 4);
-        if (tc::elect_one()) {
+    float acc[64], v[32];
 #pragma unroll
-          for (int jj = 0; jj < 2; ++jj) {
-            const uint32_t a = a0 + jj * (A_TILE >> 4), b = b0 + jj * 4;  // B: second channel block = +64 bytes inside the row
-            umma<F>(d, a, HI, b, HI, ID128, (jj | in_win) != 0 ? 1u : 0u);      // hi, first half of the block  x [W_hi; W_lo]
-            umma<F>(d, a + 2, HI, b + 2, HI, ID128, 1u);                         // hi, second half
-            umma<F>(d + 64, a + 4, HI, b, HI, ID64, 1u);                         // lo, first half  x W_hi
-            umma<F>(d + 64, a + 6, HI, b + 2, HI, ID64, 1u);                     // lo, second half
-          }
-          tc::umma_commit(&empty_bar[s]);
-        }
-        __syncwarp();
-        if (++s == STAGES) { s = 0; ph ^= 1; }
-        ++in_win;
-        if (in_win == P.win || kb == nk - 1) {
-          if (tc::elect_one()) tc::umma_commit(&tfull_bar[acc]);
-          __syncwarp();
-          in_win = 0;
-          if (++acc == 2) { acc = 0; pa ^= 1; }
-        }
-      }
-    }
-  } else {
-    // ===================== drain + epilogue =====================
-    const int q = warp & 3;              // TMEM lane quarter
-    const int g = (warp - 2) >> 2;       // column half: couts [32g, 32g + 32) of the N tile
-    int acc = 0; uint32_t pa = 0;
-    const int nwin = (nk + P.win - 1) / P.win;
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    int s = 0; uint32_t ph = 0;
     for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
       int pt, nt; tile_index(P, pixel_tiles, t, pt, nt);
       const int b = pt / (P.tiles_y * P.tiles_x), r = pt - b * (P.tiles_y * P.tiles_x);
       const int y0 = (r / P.tiles_x) * TY, x0 = (r % P.tiles_x) * TX;
-      const int m = q * 32 + lane;
-      const int y = y0 + m / TX, x = x0 + m % TX;
-      const bool inside = (y < P.H) && (x < P.W);
-      float v[32];
 #pragma unroll
       for (int i = 0; i < 32; ++i) v[i] = 0.f;
-      for (int w = 0; w < nwin; ++w) {
-        tc::mbar_wait(&tfull_bar[acc], pa);
-        tc::tc_fence_after();
-        const uint32_t t_addr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>(acc * 128 + g * 32);
-        uint32_t rm[32], rc[32];
-        tc::tmem_ld_32x32b_x32(t_addr, rm);
-        tc::tmem_ld_32x32b_x32(t_addr + 64, rc);
-        tc::tmem_ld_wait();
-        tc::tc_fence_before();
-        __syncwarp();
-        if (lane == 0) tc::mbar_arrive(&tempty_bar[acc]);
+      int in_win = 0, pend = -1;
+      for (int kb = 0; kb < nk; ++kb) {
+        tc::mbar_wait(&full_bar[s], ph);
+        const uint32_t a0 = smem_lo + static_cast<uint32_t>(s) * (STAGE >> 4) + static_cast<uint32_t>(wg * (64 * 128 >> 4));
+        const uint32_t b0 = smem_lo + static_cast<uint32_t>(s) * (STAGE >> 4) + (2 * A_TILE >> 4);
+        tc::wgmma_fence();
 #pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] += __uint_as_float(rm[i]) + __uint_as_float(rc[i]) * F::CORR;
-        if (++acc == 2) { acc = 0; pa ^= 1; }
-      }
-      const int n0 = nt * 64 + g * 32;   // GEMM column of v[0]
-      if (P.bias) {
-        const int cb = P.mode == 2 ? n0 % P.Cout : n0;
-#pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] += __ldg(P.bias + cb + i);
-      }
-      if (P.relu) {
-#pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] = fmaxf(v[i], 0.f);
-      }
-      if (inside) {
-        using E = typename F::elem;
-        constexpr int NB = 32 / F::CH, BS = 2 * F::CH;   // channel blocks held by this thread, elements per block
-        long long o;   // element offset of the channel block of n0 in the output pixel
-        if (P.mode == 2) {
-          const int tap = n0 / P.Cout, co = n0 - tap * P.Cout;
-          o = ((((long long)b * (2 * P.H) + 2 * y + (tap >> 1)) * (2LL * P.W) + 2 * x + (tap & 1)) * P.Cout + co) * 2;
+        for (int jj = 0; jj < 2; ++jj)  // B: second channel block = +64 bytes inside the weight row
+          mma_block<F>(acc, a0 + jj * (A_TILE >> 4), HI, b0 + jj * 4, HI, (jj | in_win) != 0 ? 1u : 0u);
+        tc::wgmma_commit();
+        if (++in_win == P.win || kb == nk - 1) {
+          tc::wgmma_wait<0>();
+          tc::reg_fence<64>(acc);
+          if (pend >= 0) release_stage(&empty_bar[pend]);
+          release_stage(&empty_bar[s]);
+          pend = -1;
+          drain<F>(v, acc);
+          in_win = 0;
         } else {
-          o = ((((long long)b * P.H + y) * P.W + x) * P.Cout + n0) * 2;
+          tc::wgmma_wait<1>();
+          if (pend >= 0) release_stage(&empty_bar[pend]);
+          pend = s;
         }
-        bool bad = false;
-#pragma unroll
-        for (int c = 0; c < NB; ++c) {
-          if (P.res) add_split<F>(static_cast<const E*>(P.res) + o + c * BS, v + c * F::CH);
-          if (P.res2) add_split<F>(static_cast<const E*>(P.res2) + o + c * BS, v + c * F::CH);
-          bad |= store_split<F>(static_cast<E*>(P.out) + o + c * BS, v + c * F::CH);
-        }
-        if (bad && P.flag) atomicOr(P.flag, 1);
+        if (++s == STAGES) { s = 0; ph ^= 1; }
       }
+      int y[2], x[2];
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        const int m = 64 * wg + 16 * (warp & 3) + (lane >> 2) + 8 * rr;
+        y[rr] = y0 + m / TX; x[rr] = x0 + m % TX;
+      }
+      epilogue_split<F>(P, v, b, y, x, nt * 64);
     }
   }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tc::tmem_dealloc<TMEM_COLS>(tmem_base);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// 3x3 convolution with HALO REUSE (the body layers: 97 % of a DRUNet forward).
+// 3x3 convolution with HALO REUSE (the body layers: almost all of a DRUNet forward).
 //
-// The per-tap kernel above re-reads every activation tile 9 times and every weight tile once per 128 pixels: 107 bytes per
-// clock and SM from L2 against ~50 deliverable — measured 2.0 ms per DRUNet layer where the tensor pipe needs 0.9 ms.
-// Here a CTA owns a 16 x 16-pixel tile = TWO M=128 accumulators (x-halves of 8 columns).  Per 16-channel block ONE TMA box
-// brings the (16+8) x (16+2)-position slab (tile + halo; out-of-range positions zero-filled = the convolution's padding;
-// 24 positions per slab row keep every 8-position group 1024-byte periodic) of [hi16 | lo16] rows into shared memory, and
-// the nine taps are nine shifted UMMA descriptors into it (start + ((ky*24 + kx + 8*half) * 128 B, stride between 8-row
-// groups = one slab row); the 128-byte swizzle is a function of the shared-memory address bits, so the shifted starts
-// need no base offset (validated by the bf16 halo kernel, conv_tc.cu).  A weight tile holds TWO taps of one channel block
-// ([tap even 16 ch | tap odd 16 ch] per row, rows = [W_hi; W_lo]) and is shared by both halves.
-// L2 -> SM traffic: 135 KB per channel block and 4032 tensor-pipe clocks = 33 B/clk.
-// Accumulators: per half 64 main + 64 corr columns, two buffers (512 TMEM columns); a window = `win` channel blocks.
+// The per-tap kernel above re-reads every activation tile 9 times and every weight tile once per 128 pixels.  Here a CTA
+// owns an (8 MH) x 16-pixel tile.  Per 16-channel block ONE TMA box brings the (8 MH + 8) x (16 + 2)-position slab (tile +
+// halo; out-of-range positions zero-filled = the convolution's padding; a multiple of 8 positions per slab row keeps every
+// 8-position group 1024-byte periodic) of [hi | lo] rows into shared memory, and the nine taps are nine shifted wgmma
+// descriptors into it (start + (ky * SLAB_X + kx) * 128 B, stride between 8-row groups = one slab row); the 128-byte swizzle
+// is a function of the shared-memory address bits, so the shifted starts need no base offset.  A weight tile holds TWO taps
+// of one channel block ([tap even | tap odd] per row, rows = [W_hi; W_lo]) and is shared by all consumer warpgroups.
+// Consumer warpgroup g owns the m64 block (x-half g / 2, y-half g % 2) = 8 x 8 pixels; a window = `win` channel blocks.
 // ---------------------------------------------------------------------------------------------------------------
 namespace slab {
-constexpr int TXP = 16, TYP = 16;                 // CTA pixel tile
-constexpr int SLAB_X = 24, SLAB_Y = 18;
-constexpr int SLAB_BYTES = SLAB_X * SLAB_Y * 128; // 55296
+constexpr int TYP = 16;                           // CTA pixel tile height
+constexpr int SLAB_Y = TYP + 2;
 constexpr int A_STAGES = 2, B_STAGES = 6;
 constexpr int WT_TILE = 128 * 128;
-constexpr int SMEM_BYTES = A_STAGES * SLAB_BYTES + B_STAGES * WT_TILE + 1024;
-static_assert(SLAB_BYTES % 1024 == 0, "slab stages must stay 1024-byte aligned");
-static_assert(SMEM_BYTES <= 227 * 1024, "shared memory budget");
-constexpr uint32_t TCOLS = 512;               // 2 buffers x 2 halves x (64 main + 64 corr)
+template <int MH> struct Geom {
+  static constexpr int TXP = 8 * MH;              // CTA pixel tile width
+  static constexpr int SLAB_X = TXP + 8;
+  static constexpr int SLAB_BYTES = SLAB_X * SLAB_Y * 128;
+  static constexpr int SMEM_BYTES = A_STAGES * SLAB_BYTES + B_STAGES * WT_TILE + 1024;
+  static constexpr int NWG = 2 * MH;
+  static constexpr int THREADS = 128 * NWG + 32;
+  static_assert(SLAB_BYTES % 1024 == 0, "slab stages must stay 1024-byte aligned");
+  static_assert(SMEM_BYTES <= 227 * 1024, "shared memory budget");
+};
 }  // namespace slab
 
-template <class F>
-__global__ void __launch_bounds__(THREADS, 1) conv_tc32_slab_kernel(const __grid_constant__ Maps M, const Params P) {
+template <class F, int MH>
+__global__ void __launch_bounds__(slab::Geom<MH>::THREADS, 1) conv_tc32_slab_kernel(const __grid_constant__ Maps M, const Params P) {
   using namespace slab;
+  using G = Geom<MH>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-  uint8_t* smem_b = smem + A_STAGES * SLAB_BYTES;
+  uint8_t* smem_b = smem + A_STAGES * G::SLAB_BYTES;
   __shared__ __align__(8) uint64_t afull[A_STAGES];
   __shared__ __align__(8) uint64_t aempty[A_STAGES];
   __shared__ __align__(8) uint64_t bfull[B_STAGES];
   __shared__ __align__(8) uint64_t bempty[B_STAGES];
-  __shared__ __align__(8) uint64_t tfull_bar[2];
-  __shared__ __align__(8) uint64_t tempty_bar[2];
-  __shared__ uint32_t tmem_base_smem;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int pixel_tiles = P.B * P.tiles_y * P.tiles_x;
   const int total_tiles = pixel_tiles * P.n_tiles;
   const int nblk = P.Cin / F::CH;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tc::prefetch_tmap(&M.a[0]);
     tc::prefetch_tmap(&M.b);
-    for (int s = 0; s < A_STAGES; ++s) { tc::mbar_init(&afull[s], 1); tc::mbar_init(&aempty[s], 1); }
-    for (int s = 0; s < B_STAGES; ++s) { tc::mbar_init(&bfull[s], 1); tc::mbar_init(&bempty[s], 1); }
-    for (int a = 0; a < 2; ++a) { tc::mbar_init(&tfull_bar[a], 1); tc::mbar_init(&tempty_bar[a], 8); }
+    for (int s = 0; s < A_STAGES; ++s) { tc::mbar_init(&afull[s], 1); tc::mbar_init(&aempty[s], 4 * G::NWG); }
+    for (int s = 0; s < B_STAGES; ++s) { tc::mbar_init(&bfull[s], 1); tc::mbar_init(&bempty[s], 4 * G::NWG); }
     tc::fence_barrier_init();
   }
-  if (warp == 2) tc::tmem_alloc<TCOLS>(&tmem_base_smem);
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
 
-  if (warp == 0) {
+  if (warp == 4 * G::NWG) {
     // ===================== TMA producer =====================
     if (lane == 0) {
       int sa = 0; uint32_t pha = 0;
@@ -440,179 +425,93 @@ __global__ void __launch_bounds__(THREADS, 1) conv_tc32_slab_kernel(const __grid
       for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
         int pt, nt; tile_index(P, pixel_tiles, t, pt, nt);
         const int b = pt / (P.tiles_y * P.tiles_x), r = pt - b * (P.tiles_y * P.tiles_x);
-        const int y0 = (r / P.tiles_x) * TYP, x0 = (r % P.tiles_x) * TXP;
+        const int y0 = (r / P.tiles_x) * TYP, x0 = (r % P.tiles_x) * G::TXP;
         for (int j = 0; j < nblk; ++j) {
           tc::mbar_wait(&aempty[sa], pha ^ 1);
-          if (P.dbg & 1) {
-            tc::mbar_arrive(&afull[sa]);
-          } else {
-            tc::mbar_arrive_expect_tx(&afull[sa], SLAB_BYTES);
-            tc::tma_load_4d(smem + sa * SLAB_BYTES, &M.a[0], &afull[sa], j * (2 * F::CH), x0 - 1, y0 - 1, b);
-          }
+          tc::mbar_arrive_expect_tx(&afull[sa], G::SLAB_BYTES);
+          tc::tma_load_4d(smem + sa * G::SLAB_BYTES, &M.a[0], &afull[sa], j * (2 * F::CH), x0 - 1, y0 - 1, b);
           if (++sa == A_STAGES) { sa = 0; pha ^= 1; }
           for (int tp = 0; tp < 5; ++tp) {
             tc::mbar_wait(&bempty[sb], phb ^ 1);
-            if (P.dbg & 1) {
-              tc::mbar_arrive(&bfull[sb]);
-            } else {
-              tc::mbar_arrive_expect_tx(&bfull[sb], WT_TILE);
-              tc::tma_load_2d(smem_b + sb * WT_TILE, &M.b, &bfull[sb], (j * 5 + tp) * (2 * F::CH), nt * 128);
-            }
+            tc::mbar_arrive_expect_tx(&bfull[sb], WT_TILE);
+            tc::tma_load_2d(smem_b + sb * WT_TILE, &M.b, &bfull[sb], (j * 5 + tp) * (2 * F::CH), nt * 128);
             if (++sb == B_STAGES) { sb = 0; phb ^= 1; }
           }
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    // Converged warp, one elected lane issues.  The tap loop is fully unrolled (compile-time tap shifts, one barrier wait and
-    // one commit per weight tile = 16 MMAs): the first version spent ~110 SASS instructions per tap on window / phase
-    // bookkeeping and kept the tensor pipe only 54 % busy (profiles/r02_ncu_tc32_slab_v1.csv).
-    constexpr uint32_t ID128 = F::idesc(128, 128), ID64 = F::idesc(128, 64);
-    constexpr uint32_t HI_A = tc::desc_hi_sw128(SLAB_X * 128);
+  } else {
+    // ===================== consumers =====================
+    // The tap loop is fully unrolled (compile-time tap shifts, one barrier wait and one commit per weight tile).  The group of
+    // weight tile i is committed before the group of tile i - 1 is waited for; stages are released once their group completed.
+    const int wg = warp >> 2;
+    const int half = wg >> 1, yh = wg & 1;
+    constexpr uint32_t HI_A = tc::desc_hi_sw128(G::SLAB_X * 128);
     constexpr uint32_t HI_B = tc::desc_hi_sw128(1024);
-    const uint32_t slab_lo0 = tc::smem_u32(smem) >> 4;
+    const uint32_t slab_lo0 = (tc::smem_u32(smem) >> 4) + static_cast<uint32_t>((8 * yh * G::SLAB_X + 8 * half) * 8);
     const uint32_t bt_lo0 = tc::smem_u32(smem_b) >> 4;
+    float acc[64], v[32];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
     int sa = 0; uint32_t pha = 0;
     int sb = 0; uint32_t phb = 0;
-    int acc = 0; uint32_t pa = 0;
     for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
+      int pt, nt; tile_index(P, pixel_tiles, t, pt, nt);
+      const int b = pt / (P.tiles_y * P.tiles_x), r = pt - b * (P.tiles_y * P.tiles_x);
+      const int y0 = (r / P.tiles_x) * TYP, x0 = (r % P.tiles_x) * G::TXP;
+#pragma unroll
+      for (int i = 0; i < 32; ++i) v[i] = 0.f;
       int in_win = 0;  // channel blocks accumulated in the current window
+      int pend_a = -1, pend_b = -1;
       for (int j = 0; j < nblk; ++j) {
-        if (in_win == 0) {
-          tc::mbar_wait(&tempty_bar[acc], pa ^ 1);
-        }
         tc::mbar_wait(&afull[sa], pha);
-        tc::tc_fence_after();
-        const uint32_t slab_lo = slab_lo0 + static_cast<uint32_t>(sa) * (SLAB_BYTES >> 4);
-        const uint32_t d = tmem_base + static_cast<uint32_t>(acc * 256);
+        const uint32_t slab_lo = slab_lo0 + static_cast<uint32_t>(sa) * (G::SLAB_BYTES >> 4);
         const uint32_t fresh = in_win == 0 ? 0u : 1u;
         const bool last_of_win = (in_win + 1 == P.win) || (j == nblk - 1);
 #pragma unroll
         for (int tp = 0; tp < 5; ++tp) {
           tc::mbar_wait(&bfull[sb], phb);
-          tc::tc_fence_after();
           const uint32_t b_lo = bt_lo0 + static_cast<uint32_t>(sb) * (WT_TILE >> 4);
-          if (tc::elect_one()) {
+          tc::wgmma_fence();
 #pragma unroll
-            for (int par = 0; par < 2; ++par) {
-              const int tap = 2 * tp + par;
-              if (tap < 9) {
-                const uint32_t a_t = slab_lo + static_cast<uint32_t>(((tap / 3) * SLAB_X + (tap % 3)) * 8);
-                const uint32_t b_t = b_lo + par * 4;  // odd tap: +64 bytes inside the weight row
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                  const uint32_t a = a_t + h * 64;  // x-half: 8 positions = 1024 bytes
-                  const uint32_t dh = d + h * 128;
-                  umma<F>(dh, a, HI_A, b_t, HI_B, ID128, tap == 0 ? fresh : 1u);   // hi, first half of the block  x [W_hi; W_lo]
-                  umma<F>(dh, a + 2, HI_A, b_t + 2, HI_B, ID128, 1u);              // hi, second half
-                  umma<F>(dh + 64, a + 4, HI_A, b_t, HI_B, ID64, 1u);              // lo, first half  x W_hi
-                  umma<F>(dh + 64, a + 6, HI_A, b_t + 2, HI_B, ID64, 1u);          // lo, second half
-                }
-              }
-            }
-            tc::umma_commit(&bempty[sb]);
-            if (tp == 4) {
-              tc::umma_commit(&aempty[sa]);
-              if (last_of_win) tc::umma_commit(&tfull_bar[acc]);
+          for (int par = 0; par < 2; ++par) {
+            const int tap = 2 * tp + par;
+            if (tap < 9) {
+              const uint32_t a_t = slab_lo + static_cast<uint32_t>(((tap / 3) * G::SLAB_X + (tap % 3)) * 8);
+              mma_block<F>(acc, a_t, HI_A, b_lo + par * 4, HI_B, tap == 0 ? fresh : 1u);  // odd tap: +64 bytes inside the weight row
             }
           }
-          __syncwarp();
+          tc::wgmma_commit();
+          if (tp == 4 && last_of_win) {
+            tc::wgmma_wait<0>();
+            tc::reg_fence<64>(acc);
+            if (pend_b >= 0) release_stage(&bempty[pend_b]);
+            if (pend_a >= 0) release_stage(&aempty[pend_a]);
+            release_stage(&bempty[sb]);
+            release_stage(&aempty[sa]);
+            pend_a = -1; pend_b = -1;
+            drain<F>(v, acc);
+          } else {
+            tc::wgmma_wait<1>();
+            if (pend_b >= 0) release_stage(&bempty[pend_b]);
+            if (pend_a >= 0) release_stage(&aempty[pend_a]);
+            pend_b = sb;
+            pend_a = tp == 4 ? sa : -1;
+          }
           if (++sb == B_STAGES) { sb = 0; phb ^= 1; }
         }
         if (++sa == A_STAGES) { sa = 0; pha ^= 1; }
-        if (last_of_win) {
-          in_win = 0;
-          if (++acc == 2) { acc = 0; pa ^= 1; }
-        } else {
-          ++in_win;
-        }
+        in_win = last_of_win ? 0 : in_win + 1;
       }
-    }
-  } else {
-    // ===================== drain + epilogue: group g = x-half g, TMEM lane quarter q =====================
-    const int q = warp & 3;
-    const int g = (warp - 2) >> 2;
-    int acc = 0; uint32_t pa = 0;
-    const int nwin = (nblk + P.win - 1) / P.win;
-    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
-      int pt, nt; tile_index(P, pixel_tiles, t, pt, nt);
-      const int b = pt / (P.tiles_y * P.tiles_x), r = pt - b * (P.tiles_y * P.tiles_x);
-      const int y0 = (r / P.tiles_x) * TYP, x0 = (r % P.tiles_x) * TXP;
-      const int m = q * 32 + lane;                 // GEMM row of the half: slab row m / 8, position m % 8
-      const int y = y0 + (m >> 3), x = x0 + 8 * g + (m & 7);
-      const bool inside = (y < P.H) && (x < P.W);
-      using E = typename F::elem;
-      constexpr int NB = 64 / F::CH, BS = 2 * F::CH;   // channel blocks of this thread's 64 couts, elements per block (128 bytes)
-      const long long o = ((((long long)b * P.H + y) * P.W + x) * P.Cout + nt * 64) * 2;  // element offset of this pixel's 64 channels
-      if (inside && P.res) {  // pull the residual lines towards L2 while the tile's MMAs run
+      int y[2], x[2];
 #pragma unroll
-        for (int k = 0; k < NB; ++k) asm volatile("prefetch.global.L2 [%0];" ::"l"(static_cast<const E*>(P.res) + o + k * BS));
-        if (P.res2) {
-#pragma unroll
-          for (int k = 0; k < NB; ++k) asm volatile("prefetch.global.L2 [%0];" ::"l"(static_cast<const E*>(P.res2) + o + k * BS));
-        }
+      for (int rr = 0; rr < 2; ++rr) {
+        const int m = 16 * (warp & 3) + (lane >> 2) + 8 * rr;
+        y[rr] = y0 + 8 * yh + (m >> 3); x[rr] = x0 + 8 * half + (m & 7);
       }
-      float v[64];
-#pragma unroll
-      for (int i = 0; i < 64; ++i) v[i] = 0.f;
-      for (int w = 0; w < nwin; ++w) {
-        tc::mbar_wait(&tfull_bar[acc], pa);
-        tc::tc_fence_after();
-        const uint32_t t_addr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>(acc * 256 + g * 128);
-        if (!(P.dbg & 4))
-#pragma unroll
-        for (int c0 = 0; c0 < 64; c0 += 32) {
-          uint32_t rm[32], rc[32];
-          tc::tmem_ld_32x32b_x32(t_addr + c0, rm);
-          tc::tmem_ld_32x32b_x32(t_addr + 64 + c0, rc);
-          tc::tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 32; ++i) v[c0 + i] += __uint_as_float(rm[i]) + __uint_as_float(rc[i]) * F::CORR;
-        }
-        tc::tc_fence_before();
-        __syncwarp();
-        if (lane == 0) tc::mbar_arrive(&tempty_bar[acc]);
-        if (++acc == 2) { acc = 0; pa ^= 1; }
-      }
-      const int n0 = nt * 64;
-      if (P.bias) {
-#pragma unroll
-        for (int i = 0; i < 64; ++i) v[i] += __ldg(P.bias + n0 + i);
-      }
-      if (P.relu) {
-#pragma unroll
-        for (int i = 0; i < 64; ++i) v[i] = fmaxf(v[i], 0.f);
-      }
-      if (inside && !(P.dbg & 2)) {
-        // residual operands: all loads of half of the channels (256 / 128 bytes) are issued before the first use (the first
-        // version loaded, added and stored block by block: four dependent HBM round trips per tile and thread)
-        constexpr int HB = NB / 2;   // blocks per half
-        bool bad = false;
-#pragma unroll
-        for (int cp = 0; cp < 2; ++cp) {
-          if (P.res) {
-            uint32_t raw[HB * 4][8];
-            const char* rp = reinterpret_cast<const char*>(static_cast<const E*>(P.res) + o + cp * HB * BS);
-#pragma unroll
-            for (int k = 0; k < HB * 4; ++k) tc::ldg256(rp + 32 * k, raw[k]);
-#pragma unroll
-            for (int c2 = 0; c2 < HB; ++c2) add_split_raw<F>(raw + 4 * c2, v + (cp * HB + c2) * F::CH);
-          }
-#pragma unroll
-          for (int c2 = 0; c2 < HB; ++c2) {
-            const int c = cp * HB + c2;
-            if (P.res2) add_split<F>(static_cast<const E*>(P.res2) + o + c * BS, v + c * F::CH);
-            bad |= store_split<F>(static_cast<E*>(P.out) + o + c * BS, v + c * F::CH);
-          }
-        }
-        if (bad && P.flag) atomicOr(P.flag, 1);
-      }
+      epilogue_split<F>(P, v, b, y, x, nt * 64);
     }
   }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tc::tmem_dealloc<TCOLS>(tmem_base);
 }
 
 #endif  // !DINVK_EMUL
@@ -1146,18 +1045,19 @@ static int launch(const Maps& M, const Params& P, void* stream) {
   return DINVK_POST_LAUNCH();
 }
 
-template <class F>
+template <class F, int MH>
 static int launch_slab(const Maps& M, const Params& P, void* stream) {
+  using G = slab::Geom<MH>;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(conv_tc32_slab_kernel<F>, cudaFuncAttributeMaxDynamicSharedMemorySize, slab::SMEM_BYTES);
+    cudaError_t e = cudaFuncSetAttribute(conv_tc32_slab_kernel<F, MH>, cudaFuncAttributeMaxDynamicSharedMemorySize, G::SMEM_BYTES);
     if (e != cudaSuccess) return set_error(DINVK_ECUDA, "cudaFuncSetAttribute(conv_tc32_slab): %s", cudaGetErrorString(e));
     attr_set = true;
   }
   const long long tiles = (long long)P.B * P.tiles_y * P.tiles_x * P.n_tiles;
   const int grid = (int)std::min<long long>(tiles, sm_count());
   count_launch();
-  conv_tc32_slab_kernel<F><<<grid, THREADS, slab::SMEM_BYTES, (cudaStream_t)stream>>>(M, P);
+  conv_tc32_slab_kernel<F, MH><<<grid, G::THREADS, G::SMEM_BYTES, (cudaStream_t)stream>>>(M, P);
   return DINVK_POST_LAUNCH();
 }
 
@@ -1206,12 +1106,15 @@ static int conv_generic(const void* x, const void* weight, const float* bias, co
     P.H = H; P.W = W; P.ntaps = 1; P.mode = 2; P.n_tiles = 4 * Cout / 64;
   }
   P.tiles_x = ceil_div(P.W, TX); P.tiles_y = ceil_div(P.H, TY);
-  P.dbg = 0;
   // every 2x2 layer gains from sharing the activation tile between its N tiles (down 64 -> 128: 402 -> 297 us, up 256 -> 128: 415 -> 263 us):
   // with the N tile outermost each activation byte crossed HBM n_tiles (2 .. 8) times
   P.ngrp = getenv("DINVK_TC32_NT_OUTER") ? 1 : P.n_tiles;
   return launch<F>(M, P, stream);
 }
+
+// x-halves of the slab kernel's CTA tile: 1 = 8 x 16 pixels, two consumer warpgroups.  (With 2, four warpgroups of 64
+// accumulator + 32 drain registers each do not fit the register file and spill.)
+constexpr int SLAB_MH = 1;
 
 template <class F>
 static int conv_slab(const void* x, const void* weight, const float* bias, const void* res, const void* res2, void* out, int B, int H, int W,
@@ -1225,30 +1128,28 @@ static int conv_slab(const void* x, const void* weight, const float* bias, const
   Params P;
   int rc;
   const long long px = (long long)Cin * 2 * F::EB;
-  if ((rc = make_act_map<F>(&M.a[0], x, B, H, W, Cin, px, px * W, px * W * H, slab::SLAB_X, slab::SLAB_Y))) return rc;
+  using G = slab::Geom<SLAB_MH>;
+  if ((rc = make_act_map<F>(&M.a[0], x, B, H, W, Cin, px, px * W, px * W * H, G::SLAB_X, slab::SLAB_Y))) return rc;
   M.a[1] = M.a[0]; M.a[2] = M.a[0]; M.a[3] = M.a[0];
   if ((rc = make_w_map<F>(&M.b, weight, 10LL * Cin, 2LL * Cout))) return rc;
   P.B = B; P.H = H; P.W = W; P.Cin = Cin; P.Cout = Cout;
   P.ntaps = 9; P.kc_per_tap = Cin / F::CH; P.mode = 0; P.n_tiles = Cout / 64;
   for (int t = 0; t < 9; ++t) { P.dx[t] = t % 3 - 1; P.dy[t] = t / 3 - 1; P.amap[t] = 0; }
   P.relu = act; P.res = res; P.res2 = res2; P.out = out; P.bias = bias; P.flag = flag;
-  // accumulation window in channel blocks: ONE block by default = 18 full-scale accumulations (tf32: k = 144, fp16: k = 288).
-  // The tensor core truncates its fp32 accumulator once per MMA; over a plain 20-layer chain (DnCNN) the resulting bias
-  // compounds to 5e-6 with this window and to 1e-5 with twice as many MMAs per window (tools/micro/tf32_probe.cu, DESIGN §4.4)
+  // accumulation window in channel blocks: ONE block by default = 18 full-scale accumulations (tf32: k = 144, fp16: k = 288),
+  // so that the tensor core's own fp32 accumulation only ever sees short partial sums (DESIGN §4.4)
   static const int def_win = getenv("DINVK_TC32_SLAB_WINDOW") ? std::max(1, atoi(getenv("DINVK_TC32_SLAB_WINDOW"))) : 1;
   P.win = window > 0 ? window : def_win;
-  P.tiles_x = ceil_div(W, slab::TXP); P.tiles_y = ceil_div(H, slab::TYP);
-  P.dbg = getenv("DINVK_TC32_DBG") ? atoi(getenv("DINVK_TC32_DBG")) : 0;
-  // measured (profiles/r02_tc32h_nt_order.txt): with 2 N tiles the shared slab pays (128 -> 128: 731 -> 710 us); with all 4 or 8 N tiles of a
-  // pixel tile adjacent its CTAs stream 4 or 8 different weight groups at once and the order that keeps ONE group hot wins
-  // (512 -> 512 + residual: 773 vs 803 us) — hence groups of at most 2 (DINVK_TC32_NT_GROUP overrides: 1 = N tile outermost)
+  P.tiles_x = ceil_div(W, G::TXP); P.tiles_y = ceil_div(H, slab::TYP);
+  // N tiles of a pixel tile are adjacent work items in groups of at most 2, so that CTAs sharing a slab run together while
+  // only one weight group at a time is streamed (DINVK_TC32_NT_GROUP overrides: 1 = N tile outermost)
   {
     static const int env_g = getenv("DINVK_TC32_NT_GROUP") ? atoi(getenv("DINVK_TC32_NT_GROUP")) : 0;
     int g = env_g > 0 ? env_g : (P.n_tiles <= 2 ? P.n_tiles : 1);
     while (g > 1 && P.n_tiles % g) --g;
     P.ngrp = std::max(1, std::min(g, P.n_tiles));
   }
-  return launch_slab<F>(M, P, stream);
+  return launch_slab<F, SLAB_MH>(M, P, stream);
 }
 
 #endif  // !DINVK_EMUL

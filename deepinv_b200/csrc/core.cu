@@ -30,7 +30,7 @@ int sm_count() {
     int dev = 0;
     cudaGetDevice(&dev);
     int v = 0;
-    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 148;
+    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 132;  // H100 SXM
     n = v;
   }
   return n;

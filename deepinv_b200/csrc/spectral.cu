@@ -13,7 +13,7 @@
 //   ROW pass: one CTA owns L full rows (fully contiguous), transforms along W; the mask / spectral
 //             multiplier, and for A^T A / prox the inverse row transform, are fused into this pass.
 // The intermediate between the two passes is an interleaved complex workspace written once and read
-// once; for the cfg2 batch (33.5 MB) it stays resident in the 126 MB L2.  When the multiplier does
+// once; for the cfg2 batch (33.5 MB) it stays resident in the 50 MB L2.  When the multiplier does
 // not depend on h (Cartesian line masks, mask_sh == 0) and both transforms run, the H-direction
 // transforms cancel algebraically and a single ROW pass does the whole operator.
 #include "common.cuh"

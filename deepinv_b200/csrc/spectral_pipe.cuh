@@ -1,13 +1,13 @@
 // spectral_pipe.cuh — persistent, bulk-copy-pipelined spectral kernels for 256x256 images (included by spectral.cu).
 //
 // Same arithmetic as the tile passes in spectral.cu / spectral_fast.cuh (radix-16 Stockham stages, fp64-generated
-// twiddles), restructured around what bounds the operator on B200 (DESIGN.md §4.1):
+// twiddles), restructured around what bounds the operator (DESIGN.md §4.1):
 //
 //   * HBM latency: the old passes kept < 40 KB per SM in flight (load -> barrier -> transform -> store inside each
 //     CTA).  Here every kernel is persistent (2 CTAs per SM, static round-robin over tiles) and its tiles arrive by
 //     `cp.async.bulk` (TMA 1-D bulk copies completing on an mbarrier) into a shared-memory ring filled one tile ahead,
 //     so the loads of tile i+1 are in flight while tile i is transformed and stored.
-//   * issue slots: a 256x256 fp32 FFT on B200 needs about as many issue cycles as HBM cycles.  Signs of the centred
+//   * issue slots: a 256x256 fp32 FFT needs about as many issue cycles as HBM cycles.  Signs of the centred
 //     transform, the orthonormal scale and the conjugations of the inverse are folded into per-thread constants or
 //     the twiddle tables; all indexing is compile-time; the forward -> multiplier -> inverse row pass keeps the
 //     spectrum in registers between the two transforms (the bins a thread owns after the last forward stage,

@@ -1,6 +1,6 @@
-// tc_ptx.cuh — thin inline-PTX wrappers for the Blackwell (sm_100a) tensor-core path:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 {alloc, mma, commit, ld, fence}, UMMA descriptors.
-// Formats follow the PTX ISA / CUTLASS cute/arch/mma_sm100_desc.hpp (SmemDescriptor, InstrDescriptor).
+// tc_ptx.cuh — thin inline-PTX wrappers for the Hopper (sm_90a) tensor-core path:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma {mma_async, fence, commit_group, wait_group}, shared-memory matrix descriptors.
+// Formats follow the PTX ISA (warpgroup-level matrix shared-memory layout, matrix descriptor format).
 #pragma once
 #include <cstdint>
 #include <cuda.h>
@@ -72,107 +72,133 @@ __device__ __forceinline__ void tma_load_4d(void* smem, const CUtensorMap* m, ui
       : "memory");
 }
 
-// ---- tcgen05 --------------------------------------------------------------------------------------
-template <uint32_t NCOLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem) {  // one full warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "n"(NCOLS) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// ---- wgmma (Hopper warpgroup MMA) -------------------------------------------------------------------
+// D[registers] (+)= A[smem] * B[smem], both operands K-major with the 128-byte swizzle TMA writes.  Issued by all 128
+// threads of a warpgroup; the accumulator fragment of m64nN (fp32) is N/2 registers per thread: register 4j + 2h + e
+// holds row 16 * (warp % 4) + lane / 4 + 8h, column 8j + 2 * (lane % 4) + e.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// pins the accumulator registers in program order: the compiler may not move their reads above a wgmma_wait (the wgmma
+// asm statements are the only writers it sees) nor their writes below the next wgmma
+template <int N>
+__device__ __forceinline__ void reg_fence(float* d) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-template <uint32_t NCOLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {  // same warp that allocated
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// D[tmem] (+)= A[smem] * B[smem], kind::f16 (bf16 inputs, fp32 accumulate); issued by ONE thread
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// same, descriptors passed as (lo, hi) 32-bit halves: the lo half is just (smem address >> 4) for addresses below
-// 256 KB, so successive K steps / taps are a 32-bit add of a compile-time constant on a warp-uniform value
-__device__ __forceinline__ void umma_bf16_lohi(uint32_t tmem_d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi,
-                                               uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      ".reg .b64 da, db;\n\t"
-      "mov.b64 da, {%1, %2};\n\t"
-      "mov.b64 db, {%3, %4};\n\t"
-      "setp.ne.b32 p, %6, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// high word of the K-major SWIZZLE_128B descriptor: SBO>>4 in [0,14), version=1 in [14,16), layout type 2 in [29,32)
-__host__ __device__ constexpr uint32_t desc_hi_sw128(uint32_t sbo_bytes) { return ((sbo_bytes >> 4) & 0x3FFF) | (1u << 14) | (2u << 29); }
-// make the mbarrier track completion of all MMAs issued so far by this thread (implies fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// 32 lanes x 32 consecutive 32-bit columns -> 32 registers per thread (thread t of the warp = TMEM lane base+t)
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+// Shared-memory matrix descriptor (PTX ISA "matrix descriptor" for wgmma), passed as (lo, hi) 32-bit halves:
+//   lo: [0,14) start address >> 4, [16,30) leading byte offset >> 4 (unused by swizzled K-major operands; set to 1 by the
+//       wrappers below);  hi: [0,14) stride byte offset >> 4 (distance between 8-row groups), [30,32) layout type (1 = 128B swizzle).
+// The lo half is (smem address >> 4), so successive K steps / taps are a 32-bit add of a constant on a warp-uniform value.
+// The swizzle is applied to the shared-memory ADDRESS bits on both the TMA write and the wgmma read, so start addresses
+// shifted by whole 128-byte rows or by 32-byte K steps inside a 1024-byte atom need no base offset.
+__host__ __device__ constexpr uint32_t desc_hi_sw128(uint32_t sbo_bytes) { return ((sbo_bytes >> 4) & 0x3FFF) | (1u << 30); }
 
-// ---- 256-bit global accesses (sm_100: LDG/STG.E.ENL2.256) — one full 32-byte sector per lane ---------------
+// dense wgmma shapes used by the convolutions: bf16 (m64 n16/64/128 k16), fp16 (m64 n64/128 k16), tf32 (m64 n64/128 k8)
+__device__ __forceinline__ void wgmma_bf16_n16(float* d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
+      "mov.b64 da, {%8, %9};\n\tmov.b64 db, {%10, %11};\n\tsetp.ne.b32 p, %12, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, da, db, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "r"(a_lo | (1u << 16)), "r"(a_hi), "r"(b_lo | (1u << 16)), "r"(b_hi), "r"(scale_d)
+      : "memory");
+}
+__device__ __forceinline__ void wgmma_bf16_n64(float* d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
+      "mov.b64 da, {%32, %33};\n\tmov.b64 db, {%34, %35};\n\tsetp.ne.b32 p, %36, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, da, db, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a_lo | (1u << 16)), "r"(a_hi), "r"(b_lo | (1u << 16)), "r"(b_hi), "r"(scale_d)
+      : "memory");
+}
+__device__ __forceinline__ void wgmma_bf16_n128(float* d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
+      "mov.b64 da, {%64, %65};\n\tmov.b64 db, {%66, %67};\n\tsetp.ne.b32 p, %68, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, da, db, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a_lo | (1u << 16)), "r"(a_hi), "r"(b_lo | (1u << 16)), "r"(b_hi), "r"(scale_d)
+      : "memory");
+}
+__device__ __forceinline__ void wgmma_f16_n64(float* d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
+      "mov.b64 da, {%32, %33};\n\tmov.b64 db, {%34, %35};\n\tsetp.ne.b32 p, %36, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, da, db, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a_lo | (1u << 16)), "r"(a_hi), "r"(b_lo | (1u << 16)), "r"(b_hi), "r"(scale_d)
+      : "memory");
+}
+__device__ __forceinline__ void wgmma_f16_n128(float* d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
+      "mov.b64 da, {%64, %65};\n\tmov.b64 db, {%66, %67};\n\tsetp.ne.b32 p, %68, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, da, db, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a_lo | (1u << 16)), "r"(a_hi), "r"(b_lo | (1u << 16)), "r"(b_hi), "r"(scale_d)
+      : "memory");
+}
+__device__ __forceinline__ void wgmma_tf32_n64(float* d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
+      "mov.b64 da, {%32, %33};\n\tmov.b64 db, {%34, %35};\n\tsetp.ne.b32 p, %36, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, da, db, p, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a_lo | (1u << 16)), "r"(a_hi), "r"(b_lo | (1u << 16)), "r"(b_hi), "r"(scale_d)
+      : "memory");
+}
+__device__ __forceinline__ void wgmma_tf32_n128(float* d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
+      "mov.b64 da, {%64, %65};\n\tmov.b64 db, {%66, %67};\n\tsetp.ne.b32 p, %68, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, da, db, p, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a_lo | (1u << 16)), "r"(a_hi), "r"(b_lo | (1u << 16)), "r"(b_hi), "r"(scale_d)
+      : "memory");
+}
+
+// ---- 256-bit global accesses as two 128-bit ones: one full 32-byte sector per lane ---------------------
 __device__ __forceinline__ void ldg256(const void* p, uint32_t (&r)[8]) {
-  asm volatile("ld.global.nc.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "l"(p));
+  const uint4 a = __ldg(reinterpret_cast<const uint4*>(p)), b = __ldg(reinterpret_cast<const uint4*>(p) + 1);
+  r[0] = a.x; r[1] = a.y; r[2] = a.z; r[3] = a.w; r[4] = b.x; r[5] = b.y; r[6] = b.z; r[7] = b.w;
 }
 __device__ __forceinline__ void stg256(void* p, const uint32_t (&r)[8]) {
-  asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]),
-               "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-
-// ---- descriptors ------------------------------------------------------------------------------------
-// shared-memory matrix descriptor, K-major operand stored as rows of 128 bytes (64 bf16) with the 128-byte
-// swizzle TMA writes; 8-row groups are `sbo_bytes` apart (1024 for a dense tile).  Layout of the 64 bits
-// (cute::UMMA::SmemDescriptor): [0,14) start>>4, [16,30) LBO>>4, [32,46) SBO>>4, [46,48) version=1,
-// [49,52) base offset, [61,64) layout type (2 = SWIZZLE_128B).
-__device__ __forceinline__ uint64_t make_desc_sw128(uint32_t smem_addr, uint32_t sbo_bytes, uint32_t base_offset = 0) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFF);
-  d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(base_offset & 7) << 49;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
-}
-// instruction descriptor for kind::f16 with BF16 A/B (K-major both), FP32 accumulate (cute::UMMA::InstrDescriptor):
-// [4,6) c_format=1 (F32), [7,10) a_format=1 (BF16), [10,13) b_format=1, [15] a_major=0, [16] b_major=0,
-// [17,23) N>>3, [24,29) M>>4
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(N >> 3) << 17) | (static_cast<uint32_t>(M >> 4) << 24);
+  reinterpret_cast<uint4*>(p)[0] = make_uint4(r[0], r[1], r[2], r[3]);
+  reinterpret_cast<uint4*>(p)[1] = make_uint4(r[4], r[5], r[6], r[7]);
 }
 
 }  // namespace tc

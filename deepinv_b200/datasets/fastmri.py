@@ -9,7 +9,7 @@ Volumes: fastMRI `.h5` files when `h5py` is importable (like the reference, whic
 "HDF5-shaped" `.npz` volumes with the same keys (`kspace` complex64 (D, (N,) H, W), optional `reconstruction_rss` /
 `reconstruction_esc` (D, h, w), optional `mask` (W,), optional `attrs__num_low_frequency`) — the container this image can read.
 
-B200 path: `load_batch(indices, device)` stages the raw INTERLEAVED complex slices in one pinned host buffer, moves them
+GPU path: `load_batch(indices, device)` stages the raw INTERLEAVED complex slices in one pinned host buffer, moves them
 with a single asynchronous copy and de-interleaves on the device (`dinvk_interleaved_to_planar`): the reference's host-side
 `view_as_real + moveaxis + contiguous` pass per slice (mixins.py:148-156) and the per-sample H2D copies of a default
 DataLoader do not exist; file masks come back as a `(B, W)` device tensor (`line_mask` expands them to the `(B, 2, H, W)` view
@@ -197,7 +197,7 @@ class FastMRISliceDataset(torch.utils.data.Dataset):
             target, kspace, params = self.transform(target, kspace, seed=str(fname) + str(slice_ind), metadata=metadata, **params)
         return (target if target is not None else torch.nan, kspace) + ((params,) if params else ())
 
-    # ---- B200 path ----------------------------------------------------------------------------------------------------
+    # ---- GPU path -----------------------------------------------------------------------------------------------------
     def load_batch(self, indices, device, non_blocking: bool = True) -> dict:
         """slices `indices` (same k-space shape) -> {"y": (B, 2, (N,) H, W) fp32 on `device`, "mask": (B, W) fp32 or None,
         "target": list of host tensors / None}.  One pinned staging buffer, one H2D copy, de-interleave on the device."""

@@ -5,7 +5,7 @@ Drop-in for deepinv/models/drunet.py:23-263: same constructor, same module tree 
 `load_state_dict`), same `forward(x, sigma)` noise-level handling (:212-249), same padding / split
 rules for awkward sizes (:252-262, models/utils.py:49-101).  The nn.Conv2d / ConvTranspose2d modules
 below only hold the parameters; the arithmetic is `dinvk_conv_f32` (fp32 parity path) or the
-tcgen05 bf16 implicit GEMM (`precision="bf16"`, see deepinv_b200/models/tc_engine.py).
+wgmma bf16 implicit GEMM (`precision="bf16"`, see deepinv_b200/models/tc_engine.py).
 
 Layer list for the reference configuration (SURVEY Appendix A.12): head 3x3, 4 scales of 4 ResBlocks
 (x + conv(relu(conv(x)))) with 2x2/s2 down-convs, 4 body ResBlocks, 2x2/s2 transposed up-convs with

@@ -1,6 +1,6 @@
 """bf16 tensor-core execution of DRUNet / DnCNN (precision="bf16").
 
-Activations stay NHWC bf16 in HBM between layers; every 3x3 convolution is one launch of the tcgen05
+Activations stay NHWC bf16 in HBM between layers; every 3x3 convolution is one launch of the wgmma
 implicit-GEMM kernel (csrc/conv_tc.cu) with ReLU / residual / U-Net-skip additions fused into its
 epilogue; the network tail writes fp32 NCHW directly.  Weights are repacked once per parameter version
 into the K-major (Cout, taps*Cin) bf16 layout the kernel's TMA descriptors expect.

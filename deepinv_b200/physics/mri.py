@@ -1,4 +1,4 @@
-"""MRI / MultiCoilMRI on the fused sm_100a spectral kernels.
+"""MRI / MultiCoilMRI on the fused sm_90a spectral kernels.
 
 Drop-in for deepinv/physics/mri.py:11-695 (2-D and 2-D+t: MRI, MultiCoilMRI, DynamicMRI, SequentialMRI; single-coil
 `three_d=True` runs the separable 3-D transform on the 2-D kernels — a correctness-level path; 3-D multi-coil is out of scope).  Same constructor, buffers (`mask`, `coil_maps`), kwargs-store-as-buffer side

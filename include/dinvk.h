@@ -1,5 +1,5 @@
 /*
- * dinvk.h — C ABI of libdinvk.so, the sm_100a kernel library behind the
+ * dinvk.h — C ABI of libdinvk.so, the sm_90a kernel library behind the
  * deepinv_b200 drop-in physics operators / optim steps / denoisers.
  *
  * The reference (deepinv v0.4.1) is pure Python over ATen: it has no FFI of its
@@ -242,7 +242,7 @@ int dinvk_conv_f32_wgrad(const float* x, const float* xadd, const float* gout, f
 /* gin = gout * [out > 0] : backward of the fused ReLU, `out` being the forward output */
 int dinvk_relu_bwd(const float* gout, const float* out, float* gin, long long n, void* stream);
 
-/* bf16 tensor-core path (tcgen05 implicit GEMM, TMA-fed), NHWC bf16 activations:
+/* bf16 tensor-core path (wgmma implicit GEMM, TMA-fed), NHWC bf16 activations:
  *   x (B,H,W,Cin) bf16, weight (Cout, 9*Cin) bf16 K-major with k = (ky*3+kx)*Cin + c,
  *   out (B,H,W,Cout) bf16;  out = act(conv3x3(x) + bias) + res + res2   (bias fp32 (Cout) optional;
  *   res/res2 optional, bf16 NHWC; res2 carries the U-Net skip that the reference adds before the next
@@ -276,7 +276,7 @@ int dinvk_conv2x2_up_bf16(const void* x, const void* xadd, const void* weight, v
                           int B, int H, int W, int Cin, int Cout, void* stream);
 
 
-/* fp32-grade tensor-core path (split-operand tcgen05 implicit GEMM, TMA-fed; replaces the same ATen / cuDNN calls as
+/* fp32-grade tensor-core path (split-operand wgmma implicit GEMM, TMA-fed; replaces the same ATen / cuDNN calls as
  * dinvk_conv_f32: deepinv/models/drunet.py:200-263,323-433, dncnn.py:116-140) — every fp32 value v travels as a pair
  * (hi, lo) of narrow values, products hi*hi + hi*lo + lo*hi are accumulated in fp32 and drained to registers every `window`
  * pipeline steps (0 = library default).  Two formats (`fmt`):

@@ -23,10 +23,10 @@ SANITIZE = os.environ.get("DINVK_EMUL_SANITIZE") in ("1", "thread")
 # stand-in for compute-sanitizer's racecheck (LD_PRELOAD=$(gcc -print-file-name=libtsan.so)).
 TSAN = os.environ.get("DINVK_EMUL_SANITIZE") == "thread"
 OUT = HERE / "_build" / ("libdinvk_emul_tsan.so" if TSAN else "libdinvk_emul_asan.so" if SANITIZE else "libdinvk_emul.so")
-# SIMT-only translation units (the tcgen05/TMA kernels cannot be emulated)
+# SIMT-only translation units (the wgmma/TMA kernels cannot be emulated)
 SOURCES = ["core.cu", "spectral.cu", "elementwise.cu", "radon.cu", "blur.cu", "conv_simt.cu"]
 # conv_tc32.cu enters through tests/emul/conv_tc32_model.cu: its CUDA-core kernels (network head / tail, layout converters) as they
-# are — the tcgen05 / TMA parts are compiled out — plus a test-only scalar model of the tensor-core layers behind the same C ABI
+# are — the wgmma / TMA parts are compiled out — plus a test-only scalar model of the tensor-core layers behind the same C ABI
 EXTRA = [HERE / "conv_tc32_model.cu"]
 
 

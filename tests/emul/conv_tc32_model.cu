@@ -3,7 +3,7 @@
 // (deepinv_b200/models/tc_engine.py: packing orders, residual / skip wiring, overflow flag) can run end to end on the host emulation.
 // The model implements the C-ABI contract of dinvk_conv_tc32 / dinvk_conv_tc32_slab — operands as (hi, lo) pairs, the three products
 // hi*hi + hi*lo + lo*hi accumulated per output, bias / ReLU / residual epilogue through the product's own store_split / add_split —
-// with plain loops; it shares NO code with the tcgen05 kernels and says nothing about them (those are tested on the B200,
+// with plain loops; it shares NO code with the wgmma kernels and says nothing about them (those are tested on the H100,
 // tests/test_gpu_tc32.py).  Never linked into libdinvk.so.
 #include "../../deepinv_b200/csrc/conv_tc32.cu"
 

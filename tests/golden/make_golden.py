@@ -563,15 +563,69 @@ def fastmri_fixture():
     save("fastmri_synth", **out)
 
 
+def callers_fixture():
+    """what the reference's own optimisers, sampler and least-squares solvers return on the inputs of optim_mri_tiny,
+    ddrm_mri_tiny and blur_gauss_circular_prox (tests/test_reference_callers_dropin.py compares the drop-in classes with it)"""
+    from deepinv.optim.linear import least_squares
+
+    def load(name):
+        z = np.load(OUT / f"{name}.npz")
+        arrs = {k: torch.from_numpy(np.asarray(z[k])) for k in z.files if k != "sd_from"}
+        sd = {k[4:].replace("__", "."): v for k, v in arrs.items() if k.startswith("sd__")}
+        if "sd_from" in z.files:  # the state_dict lives in another fixture
+            sd = load(str(z["sd_from"]))[1]
+        return arrs, sd
+
+    out = {}
+    go, sd = load("optim_mri_tiny")
+    den = dinv.models.DRUNet(in_channels=2, out_channels=2, nc=(8, 16, 32, 64), nb=2, pretrained=None).eval()
+    den.load_state_dict(sd, strict=True)
+    phys = MRI(mask=go["mask"], img_size=(2, 32, 32))
+    toy = lambda v, s: v * (1.0 - float(s))
+    with torch.no_grad():
+        out["pgd"] = PGD(data_fidelity=L2(), prior=PnP(den), stepsize=1.0, sigma_denoiser=0.05, max_iter=2, early_stop=False)(go["y"], phys)
+        out["hqs"] = HQS(data_fidelity=L2(), prior=PnP(toy), stepsize=0.8, sigma_denoiser=0.05, max_iter=3, early_stop=False)(go["y"], phys)
+    gd, _ = load("ddrm_mri_tiny")
+    sig = float(gd["sigma_noise"])
+    phys = MRI(mask=gd["mask"], img_size=(2, 32, 32), noise_model=dinv.physics.GaussianNoise(sigma=sig))
+    it = iter(list(gd["noises"]))
+    orig = torch.randn_like
+    torch.randn_like = lambda t, **kw: next(it).to(t)
+    try:
+        out["ddrm"] = dinv.sampling.DDRM(denoiser=lambda v, s: v * (1.0 / (1.0 + float(s))), sigmas=gd["sigmas"].numpy())(gd["y"], phys)
+    finally:
+        torch.randn_like = orig
+    gb, _ = load("blur_gauss_circular_prox")
+    gam = float(gb["gamma"])
+    circ = Blur(filter=gb["filt"], padding="circular")
+    valid = Blur(filter=gb["filt"], padding="valid")
+    ls = lambda p, y, **kw: least_squares(p.A, p.A_adjoint, y, parallel_dim=[0], AAT=p.A_A_adjoint, ATA=p.A_adjoint_A, **kw)
+    for solver in ("CG", "BiCGStab"):
+        out[f"ls_{solver}"] = ls(circ, gb["y"], z=gb["z"], init=gb["z"], gamma=gam, max_iter=25, tol=1e-5, solver=solver)
+    yv = valid.A(gb["z"])
+    out["yv"] = yv
+    out["ls_BiCGStab_valid"] = ls(valid, yv, z=gb["z"], init=gb["z"], gamma=gam, max_iter=25, tol=1e-5, solver="BiCGStab")
+    yn = yv + 0.01 * torch.randn(yv.shape, generator=torch.Generator().manual_seed(0))
+    out["y_lsqr"] = yn
+    out["lsqr_scalar"] = least_squares(valid.A, valid.A_adjoint, yn, z=gb["x"], init=gb["x"], gamma=2.0, parallel_dim=[0], max_iter=30,
+                                       tol=1e-6, solver="lsqr")
+    out["lsqr_batched"] = least_squares(valid.A, valid.A_adjoint, yn, z=gb["x"], init=gb["x"], gamma=torch.tensor([0.5, 3.0]),
+                                        parallel_dim=[0], max_iter=30, tol=1e-6, solver="lsqr")
+    out["minres_valid"] = ls(valid, yv, z=gb["x"], init=gb["x"], gamma=2.0, max_iter=30, tol=1e-6, solver="minres")
+    out["minres_circ"] = ls(circ, gb["y"], z=gb["z"], init=gb["z"], gamma=2.0, max_iter=15, tol=1e-6, solver="minres")
+    save("callers_dropin", **out)
+
+
 if __name__ == "__main__":
     torch.set_num_threads(8)
-    which = sys.argv[1:] or ["mri", "multicoil", "tomo", "blur", "blurfft", "model", "optim", "ddrm", "optim2", "train", "dynamic", "down", "combine", "maskgen", "mri3d", "fan", "anderson", "diffpir", "inpainting", "fastmri"]
+    which = sys.argv[1:] or ["mri", "multicoil", "tomo", "blur", "blurfft", "model", "optim", "ddrm", "optim2", "train", "dynamic", "down", "combine", "maskgen", "mri3d", "fan", "anderson", "diffpir", "inpainting", "fastmri", "callers"]
     table = {"mri": mri_fixtures, "multicoil": multicoil_fixtures, "tomo": tomo_fixtures, "blur": blur_fixtures,
              "blurfft": blurfft_fixtures, "model": model_fixtures, "optim": optim_fixtures, "ddrm": ddrm_fixture,
              "optim2": optim2_fixtures, "train": train_fixtures,
              "dynamic": dynamic_fixtures, "down": down_fixtures,
              "combine": combine_fixtures, "maskgen": maskgen_fixtures,
              "mri3d": mri3d_fixture, "fan": fanbeam_fixtures, "anderson": anderson_fixtures,
-             "diffpir": diffpir_fixture, "inpainting": inpainting_fixture, "fastmri": fastmri_fixture}
+             "diffpir": diffpir_fixture, "inpainting": inpainting_fixture, "fastmri": fastmri_fixture,
+             "callers": callers_fixture}
     for w in which:
         table[w]()

@@ -61,8 +61,8 @@ def test_clock_sampler_selects_the_window():
 
 
 def test_bench_line_contract_of_the_committed_profile():
-    """the last bench line measured on the B200 (profiles/) carries every key of the contract"""
-    line = json.loads((ROOT / "profiles" / "r02_final_bench.json").read_text())
+    """the bench line measured on the H100 (profiles/) carries every key of the contract"""
+    line = json.loads((ROOT / "profiles" / "bench_h100.json").read_text())
     for k in ("metric", "value", "unit", "n_gpus", "steps", "warmup", "ms_per_step", "higher_is_better", "scaling", "vs_baseline",
               "dtype", "data", "config", "e2e", "gpu_launches", "clocks", "roofline", "cpu_baseline"):
         assert k in line, k
@@ -90,7 +90,7 @@ def test_binding_roofline_picks_the_algorithmic_bound():
 
 
 def test_gpu_session_scripts_parse():
-    """the shell drivers of the GPU sessions (tools/*.sh) are only ever executed on the B200 box: at least their syntax is checked here"""
+    """the shell drivers of the GPU sessions (tools/*.sh) need a GPU machine: at least their syntax is checked here"""
     import subprocess
 
     for sh in sorted((ROOT / "tools").glob("*.sh")):

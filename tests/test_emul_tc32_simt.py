@@ -3,7 +3,7 @@ layout, `head64_tc32_kernel` with lanes = output channels and the thread-per-pix
 NCHW fp32, `tail64_tc32_kernel` with lanes = input channels + the transposing shuffle reduction, and the shared-memory first
 version) and the layout converters, for both split formats (fmt 0: tf32 words, fmt 1: fp16 words).  Checked against
 torch's conv2d in fp64 — the layers deepinv/models/drunet.py:150-176 (m_head / m_tail) and dncnn.py:94-131 (in_conv /
-out_conv + x) put at the ends of the networks.  The tcgen05 body layers need a B200 (tests/test_gpu_tc32.py)."""
+out_conv + x) put at the ends of the networks.  The wgmma body layers need an H100 (tests/test_gpu_tc32.py)."""
 import ctypes as C
 import os
 
@@ -137,8 +137,8 @@ def test_head_fp16_overflow_raises_the_flag():
 # ---------------------------------------------------------------------------------------------------------------------------
 # The package's fp32-grade denoiser ENGINES on the host: tc_engine.py (weight packing, ResBlock / skip wiring, per-call overflow
 # flag) driving the emulated head / tail kernels and the scalar model of the tensor-core layers (tests/emul/conv_tc32_model.cu),
-# against the oracle's fp32 networks (drunet.py:200-263, dncnn.py:116-140).  What this pins is the HOST logic; the tcgen05 kernels
-# behind the same ABI are compared with the same oracle on the B200 (tests/test_gpu_tc32.py).
+# against the oracle's fp32 networks (drunet.py:200-263, dncnn.py:116-140).  What this pins is the HOST logic; the wgmma kernels
+# behind the same ABI are compared with the same oracle on the H100 (tests/test_gpu_tc32.py).
 # ---------------------------------------------------------------------------------------------------------------------------
 @pytest.fixture()
 def emul_backend(monkeypatch):

@@ -1,4 +1,4 @@
-"""GPU tests of the bf16 tensor-core (tcgen05 + TMA) denoiser path against the oracle's fp32 ATen convolutions.
+"""GPU tests of the bf16 tensor-core (wgmma + TMA) denoiser path against the oracle's fp32 ATen convolutions.
 Tolerance: bf16 operands with fp32 accumulation give ~2^-9 relative error per product; a single layer must agree to
 5e-3 relative L2 with the fp32 result computed from the SAME bf16-rounded operands to 2e-3, and a whole
 network to 3e-2 (stated per test)."""

@@ -1,4 +1,4 @@
-"""GPU tests of the fp32-grade tensor-core denoiser path (precision="tc32": 3 x TF32 split operands on tcgen05,
+"""GPU tests of the fp32-grade tensor-core denoiser path (precision="tc32": 3 x TF32 split operands on wgmma,
 csrc/conv_tc32.cu) against fp64 / fp32 ATen convolutions and the oracle.
 
 Tolerance: the north star's 1e-5 relative L2 for whole networks and PnP loops (the reference computes these in fp32:
@@ -115,7 +115,7 @@ def test_conv3x3_tc32_positive_sums_no_bias(dev):
     x = torch.rand(1, 512, 16, 16, generator=gen) + 0.5
     w = (torch.rand(64, 512, 3, 3, generator=gen) + 0.5) / 4608
     ref64 = F.conv2d(x.double(), w.double(), padding=1)
-    # (never drained: -3.4e-5 at this K, tools/micro/tf32_probe.cu; the bias grows with the MMAs per accumulation window)
+    # (a truncating accumulator biases the result negatively; the bias grows with the MMAs per accumulation window)
     for fn, pack, kw, lim in ((ops.conv_tc32, _pack3x3_tc32, dict(window=2), 4e-7),            # k = 64 per window
                               (ops.conv_tc32_slab, _pack3x3_slab_tc32, dict(), 1e-6),          # default: k = 144
                               (ops.conv_tc32_slab, _pack3x3_slab_tc32, dict(window=2), 2.5e-6)):  # k = 288

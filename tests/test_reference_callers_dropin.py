@@ -1,31 +1,13 @@
-"""The drop-in boundary seen from the REFERENCE's side (SURVEY §8(b) "Callers"): the real deepinv v0.4.1 — its optimisers,
-data-fidelity terms, least-squares solver, DDRM sampler and Trainer — drives deepinv_b200's operator / denoiser classes.
-
-Only possible where the reference tree is importable (the authoring container: /root/reference + oracle/_shim), so the whole
-module is skipped elsewhere (e.g. on the GPU box).  The kernels are the host-emulated SIMT kernels (tests/emul), injected like
-in tests/test_host_logic_emul.py; nothing here is a product path."""
-import sys
-import warnings
-from pathlib import Path
-
+"""The drop-in classes against what the REFERENCE's own callers compute (SURVEY §8(b) "Callers"): deepinv v0.4.1's optimisers,
+data-fidelity terms, least-squares solvers and DDRM sampler were run on the same inputs and their results are stored in
+tests/golden/callers_dropin.npz (tests/golden/make_golden.py, callers_fixture); here the drop-in optimisers, sampler and solvers run
+on the drop-in operators and denoiser and must reproduce them.  The kernels are the host-emulated SIMT kernels (tests/emul),
+injected like in tests/test_host_logic_emul.py."""
 import pytest
 import torch
 
-ROOT = Path(__file__).resolve().parent.parent
-REF = Path("/root/reference")
-if not (REF / "deepinv" / "__init__.py").exists():
-    pytest.skip("reference tree not available", allow_module_level=True)
-for p in (str(ROOT / "oracle" / "_shim"), str(REF)):
-    if p not in sys.path:
-        sys.path.append(p)
-warnings.filterwarnings("ignore")
-try:
-    import deepinv as ref  # noqa: E402  the REAL reference
-except Exception as e:  # pragma: no cover
-    pytest.skip(f"reference not importable: {e}", allow_module_level=True)
-
-import parity_cases as P  # noqa: E402
-from conftest import load_golden, rel_err  # noqa: E402
+import parity_cases as P
+from conftest import load_golden, rel_err
 
 DEV = torch.device("cpu")
 
@@ -51,112 +33,65 @@ def emul_backend(monkeypatch):
 
 
 def test_reference_pgd_and_hqs_drive_dropin_mri_and_denoiser():
-    """reference BaseOptim / L2.grad / L2.prox / PnP.prox -> deepinv_b200 MRI.A, A_adjoint, A_adjoint_A, prox_l2, DRUNet; the
-    yardstick is the same reference algorithm on the reference's own MRI and DRUNet (same weights).  Two PGD iterations with the
-    real denoiser, HQS with a closed-form toy denoiser: keeps the emulated run short."""
+    """PGD / L2 / PnP over deepinv_b200 MRI.A, A_adjoint, A_adjoint_A, prox_l2 and DRUNet == the reference's PGD on its own MRI and
+    DRUNet (same weights); HQS with a closed-form toy denoiser likewise.  Two PGD iterations with the real denoiser keep the
+    emulated run short."""
     import deepinv_b200 as dinv
 
     g = load_golden("optim_mri_tiny")
+    want = load_golden("callers_dropin")
     den = P.load_model(dinv.models.DRUNet, g, DEV, in_channels=2, out_channels=2, nc=(8, 16, 32, 64), nb=2)
-    refden = ref.models.DRUNet(in_channels=2, out_channels=2, nc=(8, 16, 32, 64), nb=2, pretrained=None).eval()
-    refden.load_state_dict(g["sd"], strict=True)
     phys = dinv.physics.MRI(mask=g["mask"], img_size=(2, 32, 32), device=DEV)
-    refphys = ref.physics.MRI(mask=g["mask"], img_size=(2, 32, 32))
-    pgd = lambda d: ref.optim.PGD(data_fidelity=ref.optim.L2(), prior=ref.optim.PnP(d), stepsize=1.0, sigma_denoiser=0.05,
-                                  max_iter=2, early_stop=False)
     toy = lambda v, s: v * (1.0 - float(s))
-    hqs = lambda: ref.optim.HQS(data_fidelity=ref.optim.L2(), prior=ref.optim.PnP(toy), stepsize=0.8, sigma_denoiser=0.05,
-                                max_iter=3, early_stop=False)
+    pgd = dinv.optim.PGD(data_fidelity=dinv.optim.L2(), prior=dinv.optim.PnP(den), stepsize=1.0, sigma_denoiser=0.05, max_iter=2,
+                         early_stop=False)
+    hqs = dinv.optim.HQS(data_fidelity=dinv.optim.L2(), prior=dinv.optim.PnP(toy), stepsize=0.8, sigma_denoiser=0.05, max_iter=3,
+                         early_stop=False)
     with torch.no_grad():
-        assert rel_err(pgd(den)(g["y"], phys), pgd(refden)(g["y"], refphys)) < 1e-5
-        assert rel_err(hqs()(g["y"], phys), hqs()(g["y"], refphys)) < 1e-5
+        assert rel_err(pgd(g["y"], phys), want["pgd"]) < 1e-5
+        assert rel_err(hqs(g["y"], phys), want["hqs"]) < 1e-5
 
 
 def test_reference_least_squares_solver_drives_dropin_blur():
-    """reference conjugate_gradient / least_squares (optim/linear) -> deepinv_b200 Blur.A, A_adjoint, A_adjoint_A"""
+    """conjugate gradient on the normal equations through deepinv_b200 Blur.A, A_adjoint, A_adjoint_A == the reference's prox_l2"""
     import deepinv_b200 as dinv
-    from deepinv.optim.linear import least_squares
 
     g = load_golden("blur_gauss_circular_prox")
     phys = dinv.physics.Blur(filter=g["filt"], padding="circular", device=DEV)
-    out = least_squares(phys.A, phys.A_adjoint, g["y"], z=g["z"], init=g["z"], gamma=float(g["gamma"]), parallel_dim=[0],
-                        AAT=phys.A_A_adjoint, ATA=phys.A_adjoint_A, max_iter=50, tol=1e-4, solver="CG")
+    out = dinv.optim.least_squares(phys, g["y"], z=g["z"], init=g["z"], gamma=float(g["gamma"]), solver="CG", max_iter=50, tol=1e-4)
     assert rel_err(out, g["prox"]) < 1e-4
 
 
 def test_reference_ddrm_drives_dropin_mri():
-    """reference DDRM (sampling/diffusion.py:149-224) -> deepinv_b200 MRI.U_adjoint / V / V_adjoint / mask; same sampler on the
-    reference's MRI as yardstick, recorded noise draws, closed-form toy denoiser"""
+    """DDRM (sampling/diffusion.py:149-224) over deepinv_b200 MRI.U_adjoint / V / V_adjoint / mask == the reference's DDRM on its
+    own MRI: recorded noise draws, closed-form toy denoiser"""
     import deepinv_b200 as dinv
 
     g = load_golden("ddrm_mri_tiny")
     toy = lambda v, s: v * (1.0 / (1.0 + float(s)))
     sig = float(g["sigma_noise"])
     phys = dinv.physics.MRI(mask=g["mask"], img_size=(2, 32, 32), device=DEV, noise_model=dinv.physics.GaussianNoise(sigma=sig))
-    refphys = ref.physics.MRI(mask=g["mask"], img_size=(2, 32, 32), noise_model=ref.physics.GaussianNoise(sigma=sig))
-    outs = []
-    for ph in (phys, refphys):
-        it = iter(list(g["noises"]))
-        orig = torch.randn_like
-        torch.randn_like = lambda t, **kw: next(it).to(t)
-        try:
-            outs.append(ref.sampling.DDRM(denoiser=toy, sigmas=g["sigmas"].numpy())(g["y"], ph))
-        finally:
-            torch.randn_like = orig
-    assert rel_err(outs[0], outs[1]) < 1e-5
-
-
-def test_reference_trainer_trains_dropin_unfolded_model():
-    """reference Trainer + SupLoss + PSNR (training/trainer.py) -> deepinv_b200 unfolded PGD on deepinv_b200 MRI: the
-    supervised loss goes down over the epochs and every parameter is updated"""
-    import deepinv_b200 as dinv
-    from deepinv_b200.optim import L2, Tikhonov
-    from deepinv_b200.unfolded import unfolded_builder
-
-    torch.manual_seed(0)
-    N, H, W = 8, 16, 16
-    x = torch.randn(N, 2, H, W)
-    mask = (torch.rand(1, 1, 1, W) > 0.5).float().expand(1, 2, H, W).contiguous()
-    phys = dinv.physics.MRI(mask=mask, img_size=(2, H, W), device=DEV)
-    model = unfolded_builder("PGD", params_algo={"stepsize": [0.5, 0.5], "g_param": None, "lambda": [0.3, 0.3]},
-                             trainable_params=["stepsize", "lambda"], data_fidelity=L2(), prior=Tikhonov(), max_iter=2)
-
-    class DS(torch.utils.data.Dataset):
-        def __len__(self):
-            return N
-
-        def __getitem__(self, i):
-            return x[i]
-
-    dl = torch.utils.data.DataLoader(DS(), batch_size=4)
-
-    def sup_loss():
-        with torch.no_grad():
-            return float(sum(((model(phys(xb), phys) - xb) ** 2).mean() for xb in dl))
-
-    before, p0 = sup_loss(), [p.detach().clone() for p in model.parameters()]
-    trainer = ref.Trainer(model=model, physics=phys, optimizer=torch.optim.Adam(model.parameters(), lr=1e-1), train_dataloader=dl,
-                          eval_dataloader=dl, epochs=3, losses=ref.loss.SupLoss(), online_measurements=True, device="cpu",
-                          save_path=None, verbose=False, show_progress_bar=False, plot_images=False)
-    trainer.train()
-    assert sup_loss() < before
-    assert all(not torch.equal(a, b) for a, b in zip(p0, model.parameters()))
-    res = trainer.test(dl)
-    assert "PSNR" in res and res["PSNR"] == res["PSNR"]
+    it = iter(list(g["noises"]))
+    orig = torch.randn_like
+    torch.randn_like = lambda t, **kw: next(it).to(t)
+    try:
+        out = dinv.sampling.DDRM(denoiser=toy, sigmas=g["sigmas"].numpy())(g["y"], phys)
+    finally:
+        torch.randn_like = orig
+    assert rel_err(out, load_golden("callers_dropin")["ddrm"]) < 1e-5
 
 
 @pytest.mark.parametrize("solver", ["CG", "BiCGStab"])
 def test_least_squares_solvers_match_the_reference_solvers(solver):
     """deepinv_b200.optim.least_squares (CG / BiCGStab on the kernels) == the reference's least_squares with the same solver on the
-    same (drop-in) operator: same iterates, same stopping rule"""
+    same operator (the reference's own Blur): same iterates, same stopping rule"""
     import deepinv_b200 as dinv
-    from deepinv.optim.linear import least_squares as ref_ls
 
     g = load_golden("blur_gauss_circular_prox")
+    ref = load_golden("callers_dropin")
     phys = dinv.physics.Blur(filter=g["filt"], padding="circular", device=DEV)
     gam = float(g["gamma"])
-    want = ref_ls(phys.A, phys.A_adjoint, g["y"], z=g["z"], init=g["z"], gamma=gam, parallel_dim=[0], AAT=phys.A_A_adjoint,
-                  ATA=phys.A_adjoint_A, max_iter=25, tol=1e-5, solver=solver)
+    want = ref[f"ls_{solver}"]
     got = dinv.optim.least_squares(phys, g["y"], z=g["z"], init=g["z"], gamma=gam, solver=solver, max_iter=25, tol=1e-5)
     # CG: regularised normal equations, well conditioned.  BiCGStab on this square operator: the UNregularised deblurring system
     # A x = y (see below) — 40 iterations of it amplify the round-off differences of the inner products to a few 1e-4
@@ -167,8 +102,8 @@ def test_least_squares_solvers_match_the_reference_solvers(solver):
         assert rel_err(phys.A(got), g["y"]) < 1e-3
         valid = dinv.physics.Blur(filter=g["filt"], padding="valid", device=DEV)   # rectangular: normal equations with gamma
         yv = valid.A(g["z"])
-        want_v = ref_ls(valid.A, valid.A_adjoint, yv, z=g["z"], init=g["z"], gamma=gam, parallel_dim=[0], AAT=valid.A_A_adjoint,
-                        ATA=valid.A_adjoint_A, max_iter=25, tol=1e-5, solver=solver)
+        assert rel_err(yv, ref["yv"]) < 1e-6
+        want_v = ref["ls_BiCGStab_valid"]
         got_v = dinv.optim.least_squares(valid, yv, z=g["z"], init=g["z"], gamma=gam, solver=solver, max_iter=25, tol=1e-5)
         assert rel_err(got_v, want_v) < 2e-5
 
@@ -177,13 +112,14 @@ def test_lsqr_matches_the_reference_lsqr_on_a_rectangular_operator():
     """deepinv_b200.optim.lsqr (Golub-Kahan on the kernels) vs the reference's lsqr (optim/linear/lsqr.py) on the drop-in valid-padding
     Blur (rectangular): damped problem with a warm start, and the plain pseudo-inverse"""
     import deepinv_b200 as dinv
-    from deepinv.optim.linear import least_squares as ref_ls
 
     g = load_golden("blur_gauss_circular_prox")
+    ref = load_golden("callers_dropin")
     phys = dinv.physics.Blur(filter=g["filt"], padding="valid", device=DEV)
-    y = phys.A(g["z"]) + 0.01 * torch.randn(phys.A(g["z"]).shape, generator=torch.Generator().manual_seed(0))
+    y = ref["y_lsqr"]   # the reference's valid-padding blur of z + seeded noise
+    assert rel_err(y - phys.A(g["z"]), ref["y_lsqr"] - ref["yv"]) < 1e-4
     for gam, batched in ((2.0, False), (torch.tensor([0.5, 3.0]), True)):
-        want = ref_ls(phys.A, phys.A_adjoint, y, z=g["x"], init=g["x"], gamma=gam, parallel_dim=[0], max_iter=30, tol=1e-6, solver="lsqr")
+        want = ref["lsqr_batched" if batched else "lsqr_scalar"]
         got = dinv.optim.least_squares(phys, y, z=g["x"], init=g["x"], gamma=gam, solver="lsqr", max_iter=30, tol=1e-6)
         assert rel_err(got, want) < 1e-4, batched
     cg = dinv.optim.least_squares(phys, y, z=g["x"], init=g["x"], gamma=2.0, solver="CG", max_iter=60, tol=1e-6)
@@ -194,17 +130,15 @@ def test_minres_matches_the_reference_minres():
     """deepinv_b200.optim.minres vs the reference's minres (optim/linear/minres.py): the symmetric system (A^T A + I/gamma) x = b of a
     rectangular operator through least_squares, and a symmetric complete operator handed over as A x = y"""
     import deepinv_b200 as dinv
-    from deepinv.optim.linear import least_squares as ref_ls
 
     g = load_golden("blur_gauss_circular_prox")
+    ref = load_golden("callers_dropin")
     valid = dinv.physics.Blur(filter=g["filt"], padding="valid", device=DEV)
     y = valid.A(g["z"])
-    want = ref_ls(valid.A, valid.A_adjoint, y, z=g["x"], init=g["x"], gamma=2.0, parallel_dim=[0], AAT=valid.A_A_adjoint,
-                  ATA=valid.A_adjoint_A, max_iter=30, tol=1e-6, solver="minres")
+    want = ref["minres_valid"]
     got = dinv.optim.least_squares(valid, y, z=g["x"], init=g["x"], gamma=2.0, solver="minres", max_iter=30, tol=1e-6)
     assert rel_err(got, want) < 1e-4
     circ = dinv.physics.Blur(filter=g["filt"], padding="circular", device=DEV)  # symmetric filter: A = A^T, complete system
-    want = ref_ls(circ.A, circ.A_adjoint, g["y"], z=g["z"], init=g["z"], gamma=2.0, parallel_dim=[0], AAT=circ.A_A_adjoint,
-                  ATA=circ.A_adjoint_A, max_iter=15, tol=1e-6, solver="minres")
+    want = ref["minres_circ"]
     got = dinv.optim.least_squares(circ, g["y"], z=g["z"], init=g["z"], gamma=2.0, solver="minres", max_iter=15, tol=1e-6)
     assert rel_err(got, want) < 2e-3  # unregularised deblurring: see the BiCGStab case above

@@ -1,5 +1,5 @@
 """CPU checks of the split-operand formats and of the weight packings the fp32-grade tensor-core kernels consume
-(deepinv_b200/models/tc_engine.py, csrc/conv_tc32.cu).  The kernels themselves need a B200 (tests/test_gpu_tc32.py); what can be
+(deepinv_b200/models/tc_engine.py, csrc/conv_tc32.cu).  The kernels themselves need an H100 (tests/test_gpu_tc32.py); what can be
 pinned without one is the ARITHMETIC CONTRACT they implement: every operand is hi + lo, the GEMM evaluates hi*hi + hi*lo + lo*hi, and
 the K order of each packed weight matrix matches the order in which the kernel walks taps and channel blocks.  Each test restates the
 kernel's contraction in torch (fp64 accumulation) from the PACKED tensors and compares it with the reference convolution the layer
