@@ -106,6 +106,19 @@ __device__ __forceinline__ void mma_block(float* acc, uint32_t a, uint32_t a_hi,
   mma<F, 64>(acc + 32, a + 4, a_hi, b, b_hi, 1u);        // lo, first half  x W_hi
   mma<F, 64>(acc + 32, a + 6, a_hi, b + 2, b_hi, 1u);    // lo, second half
 }
+// the same products as mma_block, as six N = 64 wgmmas on the two 32-register halves (main, corr) of acc, so that every
+// wgmma covers a whole accumulator array: ptxas serializes wgmmas when an N = 64 one updates part of an N = 128 one's
+// registers.  Per register the products and their order are those of mma_block.  W_lo is 64 rows (8 KB = 512 descriptor
+// units) after W_hi.
+template <class F>
+__device__ __forceinline__ void mma_block64(float* acc, uint32_t a, uint32_t a_hi, uint32_t b, uint32_t b_hi, uint32_t fresh) {
+  mma<F, 64>(acc, a, a_hi, b, b_hi, fresh);                  // hi, first half  x W_hi  (main)
+  mma<F, 64>(acc + 32, a, a_hi, b + 512, b_hi, fresh);       // hi, first half  x W_lo  (corr)
+  mma<F, 64>(acc, a + 2, a_hi, b + 2, b_hi, 1u);             // hi, second half x W_hi
+  mma<F, 64>(acc + 32, a + 2, a_hi, b + 514, b_hi, 1u);      // hi, second half x W_lo
+  mma<F, 64>(acc + 32, a + 4, a_hi, b, b_hi, 1u);            // lo, first half  x W_hi
+  mma<F, 64>(acc + 32, a + 6, a_hi, b + 2, b_hi, 1u);        // lo, second half x W_hi
+}
 // v[i] (row 16 * (warp % 4) + lane / 4 + 8 * ((i >> 1) & 1), column 8 * (i >> 2) + 2 * (lane % 4) + (i & 1)) += main + corr
 template <class F>
 __device__ __forceinline__ void drain(float* v, const float* acc) {
@@ -366,38 +379,41 @@ __global__ void __launch_bounds__(THREADS, 1) conv_tc32_kernel(const __grid_cons
 // 3x3 convolution with HALO REUSE (the body layers: almost all of a DRUNet forward).
 //
 // The per-tap kernel above re-reads every activation tile 9 times and every weight tile once per 128 pixels.  Here a CTA
-// owns an (8 MH) x 16-pixel tile.  Per 16-channel block ONE TMA box brings the (8 MH + 8) x (16 + 2)-position slab (tile +
-// halo; out-of-range positions zero-filled = the convolution's padding; a multiple of 8 positions per slab row keeps every
-// 8-position group 1024-byte periodic) of [hi | lo] rows into shared memory, and the nine taps are nine shifted wgmma
-// descriptors into it (start + (ky * SLAB_X + kx) * 128 B, stride between 8-row groups = one slab row); the 128-byte swizzle
-// is a function of the shared-memory address bits, so the shifted starts need no base offset.  A weight tile holds TWO taps
-// of one channel block ([tap even | tap odd] per row, rows = [W_hi; W_lo]) and is shared by all consumer warpgroups.
-// Consumer warpgroup g owns the m64 block (x-half g / 2, y-half g % 2) = 8 x 8 pixels; a window = `win` channel blocks.
+// owns a 16 x 16-pixel tile.  Per channel block ONE TMA box brings the 24 x 18-position slab (tile + halo; out-of-range
+// positions zero-filled = the convolution's padding; a multiple of 8 positions per slab row keeps every 8-position group
+// 1024-byte periodic) of [hi | lo] rows into shared memory, and the nine taps are nine shifted wgmma descriptors into it
+// (start + (ky * SLAB_X + kx) * 128 B, stride between 8-row groups = one slab row); the 128-byte swizzle is a function of the
+// shared-memory address bits, so the shifted starts need no base offset.  A weight tile holds TWO taps of one channel block
+// ([tap even | tap odd] per row, rows = [W_hi; W_lo]) and feeds all four m64 blocks of the tile: 536 bytes from L2 per pixel
+// and channel block, where an 8 x 16 tile (two m64 blocks) needs 928.
+//
+// Consumer warpgroup g owns y-half g of the tile as TWO m64 blocks (x-halves 0 and 1, 8 x 8 pixels each): 2 x (64
+// accumulator + 32 drain) registers per thread, which a full producer warpgroup makes room for through setmaxnreg.  The MMAs
+// are N = 64 wgmmas (mma_block64), which ptxas keeps in flight back to back.  Every output element sees the same products in
+// the same order, with the same drains, as with one block per warpgroup and mma_block.
 // ---------------------------------------------------------------------------------------------------------------
 namespace slab {
-constexpr int TYP = 16;                           // CTA pixel tile height
-constexpr int SLAB_Y = TYP + 2;
+constexpr int TXP = 16, TYP = 16;                 // CTA pixel tile
+constexpr int SLAB_X = TXP + 8, SLAB_Y = TYP + 2;
+constexpr int SLAB_BYTES = SLAB_X * SLAB_Y * 128;
 constexpr int A_STAGES = 2, B_STAGES = 6;
 constexpr int WT_TILE = 128 * 128;
-template <int MH> struct Geom {
-  static constexpr int TXP = 8 * MH;              // CTA pixel tile width
-  static constexpr int SLAB_X = TXP + 8;
-  static constexpr int SLAB_BYTES = SLAB_X * SLAB_Y * 128;
-  static constexpr int SMEM_BYTES = A_STAGES * SLAB_BYTES + B_STAGES * WT_TILE + 1024;
-  static constexpr int NWG = 2 * MH;
-  static constexpr int THREADS = 128 * NWG + 32;
-  static_assert(SLAB_BYTES % 1024 == 0, "slab stages must stay 1024-byte aligned");
-  static_assert(SMEM_BYTES <= 227 * 1024, "shared memory budget");
-};
+constexpr int SMEM_BYTES = A_STAGES * SLAB_BYTES + B_STAGES * WT_TILE + 1024;
+constexpr int CONSUMER_WARPS = 8;                 // two warpgroups
+constexpr int THREADS = 32 * CONSUMER_WARPS + 128; // + the producer warpgroup (one thread issues the TMA loads)
+// registers per thread after setmaxnreg: the launch gives every thread 65536 / 384 = 168; the producer warpgroup returns
+// what the consumers need for 2 x (64 + 32) live accumulator and drain floats (128 x 40 + 256 x 232 <= 65536)
+constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
+static_assert(SLAB_BYTES % 1024 == 0, "slab stages must stay 1024-byte aligned");
+static_assert(SMEM_BYTES <= 227 * 1024, "shared memory budget");
 }  // namespace slab
 
-template <class F, int MH>
-__global__ void __launch_bounds__(slab::Geom<MH>::THREADS, 1) conv_tc32_slab_kernel(const __grid_constant__ Maps M, const Params P) {
+template <class F>
+__global__ void __launch_bounds__(slab::THREADS, 1) conv_tc32_slab_kernel(const __grid_constant__ Maps M, const Params P) {
   using namespace slab;
-  using G = Geom<MH>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-  uint8_t* smem_b = smem + A_STAGES * G::SLAB_BYTES;
+  uint8_t* smem_b = smem + A_STAGES * SLAB_BYTES;
   __shared__ __align__(8) uint64_t afull[A_STAGES];
   __shared__ __align__(8) uint64_t aempty[A_STAGES];
   __shared__ __align__(8) uint64_t bfull[B_STAGES];
@@ -411,25 +427,26 @@ __global__ void __launch_bounds__(slab::Geom<MH>::THREADS, 1) conv_tc32_slab_ker
   if (threadIdx.x == 0) {
     tc::prefetch_tmap(&M.a[0]);
     tc::prefetch_tmap(&M.b);
-    for (int s = 0; s < A_STAGES; ++s) { tc::mbar_init(&afull[s], 1); tc::mbar_init(&aempty[s], 4 * G::NWG); }
-    for (int s = 0; s < B_STAGES; ++s) { tc::mbar_init(&bfull[s], 1); tc::mbar_init(&bempty[s], 4 * G::NWG); }
+    for (int s = 0; s < A_STAGES; ++s) { tc::mbar_init(&afull[s], 1); tc::mbar_init(&aempty[s], CONSUMER_WARPS); }
+    for (int s = 0; s < B_STAGES; ++s) { tc::mbar_init(&bfull[s], 1); tc::mbar_init(&bempty[s], CONSUMER_WARPS); }
     tc::fence_barrier_init();
   }
   __syncthreads();
 
-  if (warp == 4 * G::NWG) {
+  if (warp >= CONSUMER_WARPS) {
     // ===================== TMA producer =====================
-    if (lane == 0) {
+    tc::setmaxnreg_dec<PRODUCER_REGS>();
+    if (warp == CONSUMER_WARPS && lane == 0) {
       int sa = 0; uint32_t pha = 0;
       int sb = 0; uint32_t phb = 0;
       for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
         int pt, nt; tile_index(P, pixel_tiles, t, pt, nt);
         const int b = pt / (P.tiles_y * P.tiles_x), r = pt - b * (P.tiles_y * P.tiles_x);
-        const int y0 = (r / P.tiles_x) * TYP, x0 = (r % P.tiles_x) * G::TXP;
+        const int y0 = (r / P.tiles_x) * TYP, x0 = (r % P.tiles_x) * TXP;
         for (int j = 0; j < nblk; ++j) {
           tc::mbar_wait(&aempty[sa], pha ^ 1);
-          tc::mbar_arrive_expect_tx(&afull[sa], G::SLAB_BYTES);
-          tc::tma_load_4d(smem + sa * G::SLAB_BYTES, &M.a[0], &afull[sa], j * (2 * F::CH), x0 - 1, y0 - 1, b);
+          tc::mbar_arrive_expect_tx(&afull[sa], SLAB_BYTES);
+          tc::tma_load_4d(smem + sa * SLAB_BYTES, &M.a[0], &afull[sa], j * (2 * F::CH), x0 - 1, y0 - 1, b);
           if (++sa == A_STAGES) { sa = 0; pha ^= 1; }
           for (int tp = 0; tp < 5; ++tp) {
             tc::mbar_wait(&bempty[sb], phb ^ 1);
@@ -442,30 +459,35 @@ __global__ void __launch_bounds__(slab::Geom<MH>::THREADS, 1) conv_tc32_slab_ker
     }
   } else {
     // ===================== consumers =====================
-    // The tap loop is fully unrolled (compile-time tap shifts, one barrier wait and one commit per weight tile).  The group of
-    // weight tile i is committed before the group of tile i - 1 is waited for; stages are released once their group completed.
+    // The tap loop is fully unrolled (compile-time tap shifts, one barrier wait and one commit group per weight tile).  The
+    // group of weight tile i is committed before the group of tile i - 1 is waited for; stages are released once their group
+    // completed.  Every wait has a compile-time count at a fixed place in the unrolled loop and the accumulators are only
+    // read after wgmma_wait<0>: otherwise ptxas serializes every wgmma of the kernel (it then waits after each instruction).
+    tc::setmaxnreg_inc<CONSUMER_REGS>();
     const int wg = warp >> 2;
-    const int half = wg >> 1, yh = wg & 1;
-    constexpr uint32_t HI_A = tc::desc_hi_sw128(G::SLAB_X * 128);
+    constexpr uint32_t HI_A = tc::desc_hi_sw128(SLAB_X * 128);
     constexpr uint32_t HI_B = tc::desc_hi_sw128(1024);
-    const uint32_t slab_lo0 = (tc::smem_u32(smem) >> 4) + static_cast<uint32_t>((8 * yh * G::SLAB_X + 8 * half) * 8);
+    constexpr uint32_t BLK1 = 8 * 8;  // block 1 starts 8 slab positions (128 bytes = 8 descriptor units each) to the right
+    const uint32_t slab_lo0 = (tc::smem_u32(smem) >> 4) + static_cast<uint32_t>(8 * wg * SLAB_X * 8);
     const uint32_t bt_lo0 = tc::smem_u32(smem_b) >> 4;
-    float acc[64], v[32];
-#pragma unroll
-    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
     int sa = 0; uint32_t pha = 0;
     int sb = 0; uint32_t phb = 0;
     for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
       int pt, nt; tile_index(P, pixel_tiles, t, pt, nt);
       const int b = pt / (P.tiles_y * P.tiles_x), r = pt - b * (P.tiles_y * P.tiles_x);
-      const int y0 = (r / P.tiles_x) * TYP, x0 = (r % P.tiles_x) * G::TXP;
+      const int y0 = (r / P.tiles_x) * TYP, x0 = (r % P.tiles_x) * TXP;
+      // the tile's first group overwrites the accumulators (scale-d = 0); defining them here ends their live range at the
+      // last drain, so that they hold no registers during the epilogue
+      float acc0[64], acc1[64], v0[32], v1[32];
 #pragma unroll
-      for (int i = 0; i < 32; ++i) v[i] = 0.f;
+      for (int i = 0; i < 64; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; }
+#pragma unroll
+      for (int i = 0; i < 32; ++i) { v0[i] = 0.f; v1[i] = 0.f; }
       int in_win = 0;  // channel blocks accumulated in the current window
-      int pend_a = -1, pend_b = -1;
+      int pend_b = -1;
       for (int j = 0; j < nblk; ++j) {
         tc::mbar_wait(&afull[sa], pha);
-        const uint32_t slab_lo = slab_lo0 + static_cast<uint32_t>(sa) * (G::SLAB_BYTES >> 4);
+        const uint32_t slab_lo = slab_lo0 + static_cast<uint32_t>(sa) * (SLAB_BYTES >> 4);
         const uint32_t fresh = in_win == 0 ? 0u : 1u;
         const bool last_of_win = (in_win + 1 == P.win) || (j == nblk - 1);
 #pragma unroll
@@ -476,27 +498,29 @@ __global__ void __launch_bounds__(slab::Geom<MH>::THREADS, 1) conv_tc32_slab_ker
 #pragma unroll
           for (int par = 0; par < 2; ++par) {
             const int tap = 2 * tp + par;
-            if (tap < 9) {
-              const uint32_t a_t = slab_lo + static_cast<uint32_t>(((tap / 3) * G::SLAB_X + (tap % 3)) * 8);
-              mma_block<F>(acc, a_t, HI_A, b_lo + par * 4, HI_B, tap == 0 ? fresh : 1u);  // odd tap: +64 bytes inside the weight row
+            if (tap < 9) {   // odd tap: +64 bytes inside the weight row
+              const uint32_t a_t = slab_lo + static_cast<uint32_t>((tap / 3) * SLAB_X + (tap % 3)) * 8;
+              mma_block64<F>(acc0, a_t, HI_A, b_lo + par * 4, HI_B, tap == 0 ? fresh : 1u);
+              mma_block64<F>(acc1, a_t + BLK1, HI_A, b_lo + par * 4, HI_B, tap == 0 ? fresh : 1u);
             }
           }
           tc::wgmma_commit();
-          if (tp == 4 && last_of_win) {
+          if (tp == 4) {
             tc::wgmma_wait<0>();
-            tc::reg_fence<64>(acc);
+            tc::reg_fence<64>(acc0);
+            tc::reg_fence<64>(acc1);
             if (pend_b >= 0) release_stage(&bempty[pend_b]);
-            if (pend_a >= 0) release_stage(&aempty[pend_a]);
             release_stage(&bempty[sb]);
             release_stage(&aempty[sa]);
-            pend_a = -1; pend_b = -1;
-            drain<F>(v, acc);
+            pend_b = -1;
+            if (last_of_win) {
+              drain<F>(v0, acc0);
+              drain<F>(v1, acc1);
+            }
           } else {
             tc::wgmma_wait<1>();
             if (pend_b >= 0) release_stage(&bempty[pend_b]);
-            if (pend_a >= 0) release_stage(&aempty[pend_a]);
             pend_b = sb;
-            pend_a = tp == 4 ? sa : -1;
           }
           if (++sb == B_STAGES) { sb = 0; phb ^= 1; }
         }
@@ -507,9 +531,12 @@ __global__ void __launch_bounds__(slab::Geom<MH>::THREADS, 1) conv_tc32_slab_ker
 #pragma unroll
       for (int rr = 0; rr < 2; ++rr) {
         const int m = 16 * (warp & 3) + (lane >> 2) + 8 * rr;
-        y[rr] = y0 + 8 * yh + (m >> 3); x[rr] = x0 + 8 * half + (m & 7);
+        y[rr] = y0 + 8 * wg + (m >> 3); x[rr] = x0 + (m & 7);
       }
-      epilogue_split<F>(P, v, b, y, x, nt * 64);
+      epilogue_split<F>(P, v0, b, y, x, nt * 64);
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) x[rr] += 8;
+      epilogue_split<F>(P, v1, b, y, x, nt * 64);
     }
   }
 }
@@ -1045,19 +1072,18 @@ static int launch(const Maps& M, const Params& P, void* stream) {
   return DINVK_POST_LAUNCH();
 }
 
-template <class F, int MH>
+template <class F>
 static int launch_slab(const Maps& M, const Params& P, void* stream) {
-  using G = slab::Geom<MH>;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(conv_tc32_slab_kernel<F, MH>, cudaFuncAttributeMaxDynamicSharedMemorySize, G::SMEM_BYTES);
+    cudaError_t e = cudaFuncSetAttribute(conv_tc32_slab_kernel<F>, cudaFuncAttributeMaxDynamicSharedMemorySize, slab::SMEM_BYTES);
     if (e != cudaSuccess) return set_error(DINVK_ECUDA, "cudaFuncSetAttribute(conv_tc32_slab): %s", cudaGetErrorString(e));
     attr_set = true;
   }
   const long long tiles = (long long)P.B * P.tiles_y * P.tiles_x * P.n_tiles;
   const int grid = (int)std::min<long long>(tiles, sm_count());
   count_launch();
-  conv_tc32_slab_kernel<F, MH><<<grid, G::THREADS, G::SMEM_BYTES, (cudaStream_t)stream>>>(M, P);
+  conv_tc32_slab_kernel<F><<<grid, slab::THREADS, slab::SMEM_BYTES, (cudaStream_t)stream>>>(M, P);
   return DINVK_POST_LAUNCH();
 }
 
@@ -1112,10 +1138,6 @@ static int conv_generic(const void* x, const void* weight, const float* bias, co
   return launch<F>(M, P, stream);
 }
 
-// x-halves of the slab kernel's CTA tile: 1 = 8 x 16 pixels, two consumer warpgroups.  (With 2, four warpgroups of 64
-// accumulator + 32 drain registers each do not fit the register file and spill.)
-constexpr int SLAB_MH = 1;
-
 template <class F>
 static int conv_slab(const void* x, const void* weight, const float* bias, const void* res, const void* res2, void* out, int B, int H, int W,
                      int Cin, int Cout, int act, int window, int* flag, void* stream) {
@@ -1128,8 +1150,7 @@ static int conv_slab(const void* x, const void* weight, const float* bias, const
   Params P;
   int rc;
   const long long px = (long long)Cin * 2 * F::EB;
-  using G = slab::Geom<SLAB_MH>;
-  if ((rc = make_act_map<F>(&M.a[0], x, B, H, W, Cin, px, px * W, px * W * H, G::SLAB_X, slab::SLAB_Y))) return rc;
+  if ((rc = make_act_map<F>(&M.a[0], x, B, H, W, Cin, px, px * W, px * W * H, slab::SLAB_X, slab::SLAB_Y))) return rc;
   M.a[1] = M.a[0]; M.a[2] = M.a[0]; M.a[3] = M.a[0];
   if ((rc = make_w_map<F>(&M.b, weight, 10LL * Cin, 2LL * Cout))) return rc;
   P.B = B; P.H = H; P.W = W; P.Cin = Cin; P.Cout = Cout;
@@ -1140,7 +1161,7 @@ static int conv_slab(const void* x, const void* weight, const float* bias, const
   // so that the tensor core's own fp32 accumulation only ever sees short partial sums (DESIGN §4.4)
   static const int def_win = getenv("DINVK_TC32_SLAB_WINDOW") ? std::max(1, atoi(getenv("DINVK_TC32_SLAB_WINDOW"))) : 1;
   P.win = window > 0 ? window : def_win;
-  P.tiles_x = ceil_div(W, G::TXP); P.tiles_y = ceil_div(H, slab::TYP);
+  P.tiles_x = ceil_div(W, slab::TXP); P.tiles_y = ceil_div(H, slab::TYP);
   // N tiles of a pixel tile are adjacent work items in groups of at most 2, so that CTAs sharing a slab run together while
   // only one weight group at a time is streamed (DINVK_TC32_NT_GROUP overrides: 1 = N tile outermost)
   {
@@ -1149,7 +1170,7 @@ static int conv_slab(const void* x, const void* weight, const float* bias, const
     while (g > 1 && P.n_tiles % g) --g;
     P.ngrp = std::max(1, std::min(g, P.n_tiles));
   }
-  return launch_slab<F, SLAB_MH>(M, P, stream);
+  return launch_slab<F>(M, P, stream);
 }
 
 #endif  // !DINVK_EMUL

@@ -88,6 +88,14 @@ __device__ __forceinline__ void reg_fence(float* d) {
   for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
+// Moves registers between the warpgroups of a CTA: every warp of a warpgroup executes the same call; N is a multiple of 8
+// in [24, 256].  A producer warpgroup that only issues TMA gives registers back so that consumer warpgroups can hold more
+// accumulators than the launch allocation allows (65536 registers over the CTA's threads counted in whole warpgroups).
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
 // Shared-memory matrix descriptor (PTX ISA "matrix descriptor" for wgmma), passed as (lo, hi) 32-bit halves:
 //   lo: [0,14) start address >> 4, [16,30) leading byte offset >> 4 (unused by swizzled K-major operands; set to 1 by the
 //       wrappers below);  hi: [0,14) stride byte offset >> 4 (distance between 8-row groups), [30,32) layout type (1 = 128B swizzle).
