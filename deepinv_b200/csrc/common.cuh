@@ -13,6 +13,8 @@
 #include <cstdio>
 #include <cstdarg>
 #include <cmath>
+#include <algorithm>
+#include <utility>
 
 #include "../../include/dinvk.h"
 
@@ -37,6 +39,9 @@ namespace dinvk {
 char* err_buf();                 // thread-local, 512 bytes
 int set_error(int code, const char* fmt, ...);
 void count_launch();
+
+// number of SMs the grids are sized against (H100 SXM: 132); queried once on the real device
+int sm_count();
 
 #define DINVK_CHECK_ARG(cond, ...)                                  \
   do {                                                              \
@@ -67,19 +72,31 @@ void count_launch();
   }())
 #endif
 
-// opt-in to >48 KB dynamic shared memory (no-op under emulation)
+// opt-in to >48 KB dynamic shared memory (no-op under emulation).  The attribute belongs to the kernel on the current device,
+// so it is raised once per (kernel, device), and again only when a launch needs more than was set.
+int raise_smem_limit(const void* kernel, size_t bytes);
 template <typename K>
 inline int allow_smem(K kernel, size_t bytes) {
 #ifndef DINVK_EMUL
-  if (bytes > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-    if (e != cudaSuccess) return set_error(DINVK_ECUDA, "cudaFuncSetAttribute(smem=%zu): %s", bytes, cudaGetErrorString(e));
-  }
+  if (bytes > 48 * 1024) return raise_smem_limit(reinterpret_cast<const void*>(kernel), bytes);
 #else
   (void)kernel; (void)bytes;
 #endif
   return 0;
 }
+
+#ifndef DINVK_EMUL
+// persistent kernels: min(work_items, SMs) CTAs, each looping over work items
+template <typename... KArgs, typename... Args>
+inline int launch_persistent(void (*kernel)(KArgs...), int threads, int smem, long long work_items, void* stream, Args&&... args) {
+  int rc;
+  if ((rc = allow_smem(kernel, smem))) return rc;
+  const int grid = (int)std::min<long long>(work_items, sm_count());
+  count_launch();
+  kernel<<<grid, threads, smem, (cudaStream_t)stream>>>(std::forward<Args>(args)...);
+  return DINVK_POST_LAUNCH();
+}
+#endif
 
 // ---- tiny complex helpers -------------------------------------------------------------------
 __host__ __device__ __forceinline__ float2 cmul(float2 a, float2 b) {
@@ -93,8 +110,5 @@ __host__ __device__ __forceinline__ float2 csub(float2 a, float2 b) { return mak
 __host__ __device__ __forceinline__ float2 cconj(float2 a) { return make_float2(a.x, -a.y); }
 
 inline int ceil_div(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
-
-// number of SMs the grids are sized against (H100 SXM: 132); queried once on the real device
-int sm_count();
 
 }  // namespace dinvk

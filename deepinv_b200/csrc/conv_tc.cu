@@ -17,9 +17,9 @@
 //                   producer already fills the ring for the next tile.
 #include "common.cuh"
 #include "tc_ptx.cuh"
+#include "tma_tile.cuh"
 
 #include <cstdlib>
-#include <mutex>
 
 namespace dinvk {
 
@@ -636,96 +636,28 @@ __global__ void __launch_bounds__(256) conv2x2_bf16_kernel(const bf16* __restric
 }
 
 // ---- host side -------------------------------------------------------------------------------------------
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn get_encode() {
-  static EncodeTiledFn fn = nullptr;
-  static std::once_flag once;
-  std::call_once(once, []() {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess && qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(p);
-  });
-  return fn;
-}
-
-// 4-D activation view (C, X, Y, B) with arbitrary element strides (bytes) — plain NHWC for 3x3 / up, a stride-2
-// sub-lattice of the input for each tap of the 2x2 down-conv
-static int make_act_map(CUtensorMap* m, const void* ptr, int B, int Y, int X, int C, long long sx, long long sy, long long sb) {
-  EncodeTiledFn enc = get_encode();
-  if (!enc) return set_error(DINVK_ECUDA, "cuTensorMapEncodeTiled is unavailable");
-  cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)X, (cuuint64_t)Y, (cuuint64_t)B};
-  cuuint64_t strides[3] = {(cuuint64_t)sx, (cuuint64_t)sy, (cuuint64_t)sb};
-  cuuint32_t box[4] = {TC_KB, TC_TX, TC_TY, 1};
-  cuuint32_t es[4] = {1, 1, 1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return set_error(DINVK_ECUDA, "cuTensorMapEncodeTiled(activations) failed: %d", (int)r);
-  return 0;
-}
-static int make_w_map(CUtensorMap* m, const void* ptr, int K, int rows, int bn) {
-  EncodeTiledFn enc = get_encode();
-  if (!enc) return set_error(DINVK_ECUDA, "cuTensorMapEncodeTiled is unavailable");
-  cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)K * 2};
-  cuuint32_t box[2] = {TC_KB, (cuuint32_t)bn};
-  cuuint32_t es[2] = {1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return set_error(DINVK_ECUDA, "cuTensorMapEncodeTiled(weights) failed: %d", (int)r);
-  return 0;
-}
-
-template <int BN>
-static int launch_conv_tc(const TcMaps& M, const ConvTcParams& P, void* stream) {
-  using Cfg = TcCfg<BN>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
-    if (e != cudaSuccess) return set_error(DINVK_ECUDA, "cudaFuncSetAttribute(conv_tc<%d>): %s", BN, cudaGetErrorString(e));
-    attr_set = true;
-  }
-  const long long tiles = (long long)P.B * P.tiles_y * P.tiles_x * P.n_tiles;
-  const int grid = (int)std::min<long long>(tiles, sm_count());
-  count_launch();
-  conv_tc_kernel<BN><<<grid, TC_THREADS, Cfg::SMEM, (cudaStream_t)stream>>>(M, P);
-  return DINVK_POST_LAUNCH();
-}
-
-static int make_slab_map(CUtensorMap* m, const void* ptr, int B, int H, int W, int C, int slab_x) {
-  EncodeTiledFn enc = get_encode();
-  if (!enc) return set_error(DINVK_ECUDA, "cuTensorMapEncodeTiled is unavailable");
-  cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
-  cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
-  cuuint32_t box[4] = {TC_KB, (cuuint32_t)slab_x, HL_TY + 2, 1};
-  cuuint32_t es[4] = {1, 1, 1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return set_error(DINVK_ECUDA, "cuTensorMapEncodeTiled(slab) failed: %d", (int)r);
-  return 0;
+// a 128-byte-swizzled bf16 tensor map, the layout the wgmma descriptors read: box[0] = TC_KB channels = one swizzle row.
+// Weights (rows, K) K-major are 2-D maps (K, rows); NHWC activations are 4-D maps (C, X, Y, B) with byte strides.
+static int map_bf16(CUtensorMap* m, const void* ptr, int rank, const uint64_t* dims, const uint64_t* strides, const uint32_t* box,
+                    const char* what) {
+  return encode_tiled(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank, ptr, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B,
+                      CU_TENSOR_MAP_L2_PROMOTION_L2_256B, what);
 }
 
 template <int BN, bool RESIDENT, int AST, int BST, int MH>
 static int launch_conv_halo(TcMaps& M, ConvTcParams& P, const void* x, void* stream) {
   using Cfg = HaloCfg<BN, RESIDENT, AST, BST, MH>;
   using G = HaloGeom<MH>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(conv_tc_halo_kernel<BN, RESIDENT, AST, BST, MH>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
-    if (e != cudaSuccess) return set_error(DINVK_ECUDA, "cudaFuncSetAttribute(conv_tc_halo<%d>): %s", BN, cudaGetErrorString(e));
-    attr_set = true;
-  }
+  const uint64_t px = (uint64_t)P.Cin * 2;  // bytes per pixel
+  const uint64_t dims[4] = {(uint64_t)P.Cin, (uint64_t)P.W, (uint64_t)P.H, (uint64_t)P.B};
+  const uint64_t strides[3] = {px, px * P.W, px * P.W * P.H};
+  const uint32_t box[4] = {TC_KB, G::SLAB_X, HL_TY + 2, 1};
   int rc;
-  if ((rc = make_slab_map(&M.a[0], x, P.B, P.H, P.W, P.Cin, G::SLAB_X))) return rc;
+  if ((rc = map_bf16(&M.a[0], x, 4, dims, strides, box, "slab"))) return rc;
   M.a[1] = M.a[0]; M.a[2] = M.a[0]; M.a[3] = M.a[0];
   P.tiles_x = ceil_div(P.W, G::TX); P.tiles_y = ceil_div(P.H, HL_TY);
-  const long long tiles = (long long)P.B * P.tiles_y * P.tiles_x * P.n_tiles;
-  const int grid = (int)std::min<long long>(tiles, sm_count());
-  count_launch();
-  conv_tc_halo_kernel<BN, RESIDENT, AST, BST, MH><<<grid, Cfg::THREADS, Cfg::SMEM, (cudaStream_t)stream>>>(M, P);
-  return DINVK_POST_LAUNCH();
+  return launch_persistent(conv_tc_halo_kernel<BN, RESIDENT, AST, BST, MH>, Cfg::THREADS, Cfg::SMEM,
+                           (long long)P.B * P.tiles_y * P.tiles_x * P.n_tiles, stream, M, P);
 }
 
 // halo mode (DINVK_CONV_HALO): 0 = off (per-tap kernel), 1 = on (default).
@@ -742,10 +674,11 @@ static int halo_mode() {
 static int pick_bn(int rows) { return rows % 128 == 0 ? 128 : 64; }
 
 static int dispatch_conv_tc(int bn, const TcMaps& M, const ConvTcParams& P, void* stream) {
+  const long long work = (long long)P.B * P.tiles_y * P.tiles_x * P.n_tiles;
   switch (bn) {
-    case 16: return launch_conv_tc<16>(M, P, stream);
-    case 64: return launch_conv_tc<64>(M, P, stream);
-    default: return launch_conv_tc<128>(M, P, stream);
+    case 16: return launch_persistent(conv_tc_kernel<16>, TC_THREADS, TcCfg<16>::SMEM, work, stream, M, P);
+    case 64: return launch_persistent(conv_tc_kernel<64>, TC_THREADS, TcCfg<64>::SMEM, work, stream, M, P);
+    default: return launch_persistent(conv_tc_kernel<128>, TC_THREADS, TcCfg<128>::SMEM, work, stream, M, P);
   }
 }
 
@@ -760,35 +693,34 @@ static int conv3x3_tc(const void* x, const void* weight, const float* bias, cons
   DINVK_CHECK_ARG(rows % bn == 0, "conv3x3_bf16: weight rows %d not a multiple of the N tile %d", rows, bn);
   TcMaps M;
   int rc;
+  const uint64_t wdims[2] = {9ull * Cin, (uint64_t)rows}, wstride = 9ull * Cin * 2;
+  const uint32_t wbox[2] = {TC_KB, (uint32_t)bn};
+  if ((rc = map_bf16(&M.b, weight, 2, wdims, &wstride, wbox, "weights"))) return rc;
+  ConvTcParams P{};
+  P.B = B; P.H = H; P.W = W; P.Cin = Cin; P.Cout = Cout_real;
+  P.ntaps = 9; P.kc_per_tap = Cin / TC_KB;
+  for (int t = 0; t < 9; ++t) { P.dx[t] = t % 3 - 1; P.dy[t] = t / 3 - 1; }
+  P.mode = out_f32 ? 1 : 0;
+  P.n_tiles = rows / bn;
+  P.relu = act; P.res = (const bf16*)res; P.res2 = (const bf16*)res2; P.out = (bf16*)out; P.out_f32 = out_f32; P.add_f32 = add_f32; P.bias = bias;
   // slab + halo kernel (activations read once per 64-channel block instead of once per tap):
   //   64 -> 64 and the 64 -> (<=16) tail with the weights resident in shared memory; >= 128 output channels with streamed
   //   weights.  64-channel layers use 16x16-pixel CTA tiles (four m64 blocks share every weight tile), the streamed layers
-  //   8x16-pixel tiles (two m64 blocks of up to 64 accumulator registers per thread).
+  //   8x16-pixel tiles (two m64 blocks of up to 64 accumulator registers per thread).  The launcher sets tiles_x / tiles_y
+  //   from the kernel's tile geometry.
   const bool halo_tail = out_f32 && Cin == 64 && rows == 16 && !getenv("DINVK_NO_HALO_TAIL");
   const bool halo_body = !out_f32 && ((rows == 64 && Cin == 64) || bn == 128);
   if (halo_mode() != 0 && (halo_tail || halo_body)) {
-    if ((rc = make_w_map(&M.b, weight, 9 * Cin, rows, bn))) return rc;
-    ConvTcParams P;
-    P.B = B; P.H = H; P.W = W; P.Cin = Cin; P.Cout = Cout_real;
-    P.ntaps = 9; P.kc_per_tap = Cin / TC_KB;
-    for (int t = 0; t < 9; ++t) { P.dx[t] = t % 3 - 1; P.dy[t] = t / 3 - 1; P.amap[t] = 0; }
-    P.mode = out_f32 ? 1 : 0;
-    P.tiles_x = 0; P.tiles_y = 0; P.n_tiles = rows / bn;  // tiles_x/y: set by the launcher from the kernel's tile geometry
-    P.relu = act; P.res = (const bf16*)res; P.res2 = (const bf16*)res2; P.out = (bf16*)out; P.out_f32 = out_f32; P.add_f32 = add_f32; P.bias = bias;
     if (halo_tail) return launch_conv_halo<16, true, 4, 0, 1>(M, P, x, stream);
     if (bn == 64) return launch_conv_halo<64, true, 2, 0, 2>(M, P, x, stream);
     return launch_conv_halo<128, false, 2, 8, 1>(M, P, x, stream);
   }
-  if ((rc = make_act_map(&M.a[0], x, B, H, W, Cin, (long long)Cin * 2, (long long)W * Cin * 2, (long long)H * W * Cin * 2))) return rc;
+  const uint64_t px = (uint64_t)Cin * 2;
+  const uint64_t adims[4] = {(uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)B}, astrides[3] = {px, px * W, px * W * H};
+  const uint32_t abox[4] = {TC_KB, TC_TX, TC_TY, 1};
+  if ((rc = map_bf16(&M.a[0], x, 4, adims, astrides, abox, "activations"))) return rc;
   M.a[1] = M.a[0]; M.a[2] = M.a[0]; M.a[3] = M.a[0];
-  if ((rc = make_w_map(&M.b, weight, 9 * Cin, rows, bn))) return rc;
-  ConvTcParams P;
-  P.B = B; P.H = H; P.W = W; P.Cin = Cin; P.Cout = Cout_real;
-  P.ntaps = 9; P.kc_per_tap = Cin / TC_KB;
-  for (int t = 0; t < 9; ++t) { P.dx[t] = t % 3 - 1; P.dy[t] = t / 3 - 1; P.amap[t] = 0; }
-  P.mode = out_f32 ? 1 : 0;
-  P.tiles_x = ceil_div(W, TC_TX); P.tiles_y = ceil_div(H, TC_TY); P.n_tiles = rows / bn;
-  P.relu = act; P.res = (const bf16*)res; P.res2 = (const bf16*)res2; P.out = (bf16*)out; P.out_f32 = out_f32; P.add_f32 = add_f32; P.bias = bias;
+  P.tiles_x = ceil_div(W, TC_TX); P.tiles_y = ceil_div(H, TC_TY);
   return dispatch_conv_tc(bn, M, P, stream);
 }
 
@@ -798,19 +730,23 @@ static int conv2x2_down_tc(const void* x, const void* weight, void* out, int B, 
   const int Ho = H / 2, Wo = W / 2;
   const int bn = pick_bn(Cout);
   TcMaps M;
+  ConvTcParams P{};
   int rc;
+  const uint64_t px = (uint64_t)Cin * 2;
+  const uint64_t adims[4] = {(uint64_t)Cin, (uint64_t)Wo, (uint64_t)Ho, (uint64_t)B}, astrides[3] = {2 * px, 2 * px * W, px * W * H};
+  const uint32_t abox[4] = {TC_KB, TC_TX, TC_TY, 1};
   for (int t = 0; t < 4; ++t) {
-    const char* base = static_cast<const char*>(x) + ((long long)(t >> 1) * W + (t & 1)) * Cin * 2;
-    if ((rc = make_act_map(&M.a[t], base, B, Ho, Wo, Cin, 2LL * Cin * 2, 2LL * W * Cin * 2, (long long)H * W * Cin * 2))) return rc;
+    const char* base = static_cast<const char*>(x) + ((long long)(t >> 1) * W + (t & 1)) * px;
+    if ((rc = map_bf16(&M.a[t], base, 4, adims, astrides, abox, "activations"))) return rc;
+    P.amap[t] = t;
   }
-  if ((rc = make_w_map(&M.b, weight, 4 * Cin, Cout, bn))) return rc;
-  ConvTcParams P;
+  const uint64_t wdims[2] = {4ull * Cin, (uint64_t)Cout}, wstride = 4ull * Cin * 2;
+  const uint32_t wbox[2] = {TC_KB, (uint32_t)bn};
+  if ((rc = map_bf16(&M.b, weight, 2, wdims, &wstride, wbox, "weights"))) return rc;
   P.B = B; P.H = Ho; P.W = Wo; P.Cin = Cin; P.Cout = Cout;
   P.ntaps = 4; P.kc_per_tap = Cin / TC_KB;
-  for (int t = 0; t < 9; ++t) { P.dx[t] = 0; P.dy[t] = 0; P.amap[t] = t < 4 ? t : 0; }
-  P.mode = 0;
   P.tiles_x = ceil_div(Wo, TC_TX); P.tiles_y = ceil_div(Ho, TC_TY); P.n_tiles = Cout / bn;
-  P.relu = 0; P.res = nullptr; P.res2 = nullptr; P.out = (bf16*)out; P.out_f32 = nullptr; P.add_f32 = nullptr; P.bias = nullptr;
+  P.out = (bf16*)out;
   return dispatch_conv_tc(bn, M, P, stream);
 }
 
@@ -819,16 +755,20 @@ static int conv2x2_up_tc(const void* x, const void* weight, void* out, int B, in
   const int bn = pick_bn(Cout);  // an N tile never spans two taps
   TcMaps M;
   int rc;
-  if ((rc = make_act_map(&M.a[0], x, B, H, W, Cin, (long long)Cin * 2, (long long)W * Cin * 2, (long long)H * W * Cin * 2))) return rc;
+  const uint64_t px = (uint64_t)Cin * 2;
+  const uint64_t adims[4] = {(uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)B}, astrides[3] = {px, px * W, px * W * H};
+  const uint32_t abox[4] = {TC_KB, TC_TX, TC_TY, 1};
+  if ((rc = map_bf16(&M.a[0], x, 4, adims, astrides, abox, "activations"))) return rc;
   M.a[1] = M.a[0]; M.a[2] = M.a[0]; M.a[3] = M.a[0];
-  if ((rc = make_w_map(&M.b, weight, Cin, 4 * Cout, bn))) return rc;
-  ConvTcParams P;
+  const uint64_t wdims[2] = {(uint64_t)Cin, 4ull * Cout}, wstride = (uint64_t)Cin * 2;
+  const uint32_t wbox[2] = {TC_KB, (uint32_t)bn};
+  if ((rc = map_bf16(&M.b, weight, 2, wdims, &wstride, wbox, "weights"))) return rc;
+  ConvTcParams P{};
   P.B = B; P.H = H; P.W = W; P.Cin = Cin; P.Cout = Cout;
   P.ntaps = 1; P.kc_per_tap = Cin / TC_KB;
-  for (int t = 0; t < 9; ++t) { P.dx[t] = 0; P.dy[t] = 0; P.amap[t] = 0; }
   P.mode = 2;
   P.tiles_x = ceil_div(W, TC_TX); P.tiles_y = ceil_div(H, TC_TY); P.n_tiles = 4 * Cout / bn;
-  P.relu = 0; P.res = nullptr; P.res2 = nullptr; P.out = (bf16*)out; P.out_f32 = nullptr; P.add_f32 = nullptr; P.bias = nullptr;
+  P.out = (bf16*)out;
   return dispatch_conv_tc(bn, M, P, stream);
 }
 
@@ -849,17 +789,7 @@ extern "C" int dinvk_conv3x3_bf16_tail(const void* x, const void* weight16, cons
 
 template <int CT>
 static int launch_head(const HeadParams& P, void* stream) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(conv_head_kernel<CT>, cudaFuncAttributeMaxDynamicSharedMemorySize, HD_SMEM);
-    if (e != cudaSuccess) return set_error(DINVK_ECUDA, "cudaFuncSetAttribute(conv_head<%d>): %s", CT, cudaGetErrorString(e));
-    attr_set = true;
-  }
-  const long long tiles = (long long)P.B * P.tiles_y * P.tiles_x;
-  const int grid = (int)std::min<long long>(tiles, sm_count());
-  count_launch();
-  conv_head_kernel<CT><<<grid, HD_THREADS, HD_SMEM, (cudaStream_t)stream>>>(P);
-  return DINVK_POST_LAUNCH();
+  return launch_persistent(conv_head_kernel<CT>, HD_THREADS, HD_SMEM, (long long)P.B * P.tiles_y * P.tiles_x, stream, P);
 }
 
 extern "C" int dinvk_conv3x3_head_bf16(const float* x_nchw, const void* weight64, const float* bias, void* out_nhwc, int B, int C, int H,

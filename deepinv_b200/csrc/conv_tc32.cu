@@ -25,6 +25,7 @@
 #include "common.cuh"
 #ifndef DINVK_EMUL
 #include "tc_ptx.cuh"
+#include "tma_tile.cuh"
 #include <cuda_fp16.h>
 #else
 // host emulation (tests/emul): only the CUDA-core kernels of this file exist there — head, tail, layout converters; the 32-byte
@@ -38,7 +39,6 @@ inline void stg256(void* p, const uint32_t (&r)[8]) { std::memcpy(p, r, 32); }
 #include <algorithm>
 #include <cstdlib>
 #include <cstring>
-#include <mutex>
 
 namespace dinvk {
 namespace t32 {
@@ -1004,48 +1004,12 @@ __global__ void __launch_bounds__(256) nchw_to_split_kernel(const float* __restr
 
 #ifndef DINVK_EMUL
 // ---- host side -------------------------------------------------------------------------------------------
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn get_encode() {
-  static EncodeTiledFn fn = nullptr;
-  static std::once_flag once;
-  std::call_once(once, []() {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess && qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(p);
-  });
-  return fn;
-}
-
-// 4-D activation view (words, X, Y, B) of a split16 tensor with arbitrary pixel strides (bytes)
+// a 128-byte-swizzled tensor map over the split words of format F: box[0] = 2 CH words = one [hi | lo] row block.
+// Weights (rows, K) K-major are 2-D maps (K, rows); split activations are 4-D maps (words, X, Y, B) with byte pixel strides.
 template <class F>
-static int make_act_map(CUtensorMap* m, const void* ptr, int B, int Y, int X, int C, long long sx, long long sy, long long sb, int box_x,
-                        int box_y) {
-  EncodeTiledFn enc = get_encode();
-  if (!enc) return set_error(DINVK_ECUDA, "cuTensorMapEncodeTiled is unavailable");
-  cuuint64_t dims[4] = {(cuuint64_t)C * 2, (cuuint64_t)X, (cuuint64_t)Y, (cuuint64_t)B};
-  cuuint64_t strides[3] = {(cuuint64_t)sx, (cuuint64_t)sy, (cuuint64_t)sb};
-  cuuint32_t box[4] = {(cuuint32_t)(2 * F::CH), (cuuint32_t)box_x, (cuuint32_t)box_y, 1};
-  cuuint32_t es[4] = {1, 1, 1, 1};
-  CUresult r = enc(m, F::TM, 4, const_cast<void*>(ptr), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return set_error(DINVK_ECUDA, "cuTensorMapEncodeTiled(tc32 activations) failed: %d", (int)r);
-  return 0;
-}
-template <class F>
-static int make_w_map(CUtensorMap* m, const void* ptr, long long K, long long rows) {
-  EncodeTiledFn enc = get_encode();
-  if (!enc) return set_error(DINVK_ECUDA, "cuTensorMapEncodeTiled is unavailable");
-  cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)K * F::EB};
-  cuuint32_t box[2] = {(cuuint32_t)(2 * F::CH), 128};
-  cuuint32_t es[2] = {1, 1};
-  CUresult r = enc(m, F::TM, 2, const_cast<void*>(ptr), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return set_error(DINVK_ECUDA, "cuTensorMapEncodeTiled(tc32 weights) failed: %d", (int)r);
-  return 0;
+static int map_split(CUtensorMap* m, const void* ptr, int rank, const uint64_t* dims, const uint64_t* strides, const uint32_t* box,
+                     const char* what) {
+  return encode_tiled(m, F::TM, rank, ptr, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, what);
 }
 
 static int default_window() {
@@ -1055,36 +1019,6 @@ static int default_window() {
     w = e ? std::max(1, atoi(e)) : 4;
   }
   return w;
-}
-
-template <class F>
-static int launch(const Maps& M, const Params& P, void* stream) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(conv_tc32_kernel<F>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
-    if (e != cudaSuccess) return set_error(DINVK_ECUDA, "cudaFuncSetAttribute(conv_tc32): %s", cudaGetErrorString(e));
-    attr_set = true;
-  }
-  const long long tiles = (long long)P.B * P.tiles_y * P.tiles_x * P.n_tiles;
-  const int grid = (int)std::min<long long>(tiles, sm_count());
-  count_launch();
-  conv_tc32_kernel<F><<<grid, THREADS, SMEM, (cudaStream_t)stream>>>(M, P);
-  return DINVK_POST_LAUNCH();
-}
-
-template <class F>
-static int launch_slab(const Maps& M, const Params& P, void* stream) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(conv_tc32_slab_kernel<F>, cudaFuncAttributeMaxDynamicSharedMemorySize, slab::SMEM_BYTES);
-    if (e != cudaSuccess) return set_error(DINVK_ECUDA, "cudaFuncSetAttribute(conv_tc32_slab): %s", cudaGetErrorString(e));
-    attr_set = true;
-  }
-  const long long tiles = (long long)P.B * P.tiles_y * P.tiles_x * P.n_tiles;
-  const int grid = (int)std::min<long long>(tiles, sm_count());
-  count_launch();
-  conv_tc32_slab_kernel<F><<<grid, slab::THREADS, slab::SMEM_BYTES, (cudaStream_t)stream>>>(M, P);
-  return DINVK_POST_LAUNCH();
 }
 
 // kind 0: 3x3 stride 1 zero-pad 1 (weight rows = Cout/64 tiles of 128, K = 9*Cin, k = (ky*3+kx)*Cin + c)
@@ -1102,40 +1036,47 @@ static int conv_generic(const void* x, const void* weight, const float* bias, co
   DINVK_CHECK_ARG(kind == 0 || (!res && !res2), "conv_tc32: residual inputs are for kind 0 only");
   if (B == 0) return DINVK_OK;
   Maps M;
-  Params P;
+  Params P{};
   int rc;
-  const long long px = (long long)Cin * 2 * F::EB;  // bytes per input pixel
+  const uint64_t px = (uint64_t)Cin * 2 * F::EB;  // bytes per input pixel
   P.B = B; P.Cin = Cin; P.Cout = Cout;
   P.kc_per_tap = Cin / (2 * F::CH);
   P.relu = act; P.res = res; P.res2 = res2; P.out = out; P.bias = bias; P.flag = flag;
   P.win = window > 0 ? window : default_window();
-  for (int t = 0; t < 9; ++t) { P.dx[t] = 0; P.dy[t] = 0; P.amap[t] = 0; }
-  if (kind == 0) {
-    if ((rc = make_act_map<F>(&M.a[0], x, B, H, W, Cin, px, px * W, px * W * H, TX, TY))) return rc;
-    M.a[1] = M.a[0]; M.a[2] = M.a[0]; M.a[3] = M.a[0];
-    if ((rc = make_w_map<F>(&M.b, weight, 9LL * Cin, 2LL * Cout))) return rc;
-    P.H = H; P.W = W; P.ntaps = 9; P.mode = 0; P.n_tiles = Cout / 64;
-    for (int t = 0; t < 9; ++t) { P.dx[t] = t % 3 - 1; P.dy[t] = t / 3 - 1; }
-  } else if (kind == 1) {
+  const uint32_t abox[4] = {2 * F::CH, TX, TY, 1};
+  long long K = Cin, rows = 2LL * Cout;  // weight matrix (rows, K), K-major
+  if (kind == 1) {
     const int Ho = H / 2, Wo = W / 2;
+    const uint64_t adims[4] = {(uint64_t)Cin * 2, (uint64_t)Wo, (uint64_t)Ho, (uint64_t)B}, astrides[3] = {2 * px, 2 * px * W, px * W * H};
     for (int t = 0; t < 4; ++t) {
       const char* base = reinterpret_cast<const char*>(x) + ((long long)(t >> 1) * W + (t & 1)) * px;
-      if ((rc = make_act_map<F>(&M.a[t], base, B, Ho, Wo, Cin, 2 * px, 2 * px * W, px * W * H, TX, TY))) return rc;
+      if ((rc = map_split<F>(&M.a[t], base, 4, adims, astrides, abox, "tc32 activations"))) return rc;
       P.amap[t] = t;
     }
-    if ((rc = make_w_map<F>(&M.b, weight, 4LL * Cin, 2LL * Cout))) return rc;
-    P.H = Ho; P.W = Wo; P.ntaps = 4; P.mode = 0; P.n_tiles = Cout / 64;
+    K = 4LL * Cin;
+    P.H = Ho; P.W = Wo; P.ntaps = 4; P.n_tiles = Cout / 64;
   } else {
-    if ((rc = make_act_map<F>(&M.a[0], x, B, H, W, Cin, px, px * W, px * W * H, TX, TY))) return rc;
+    const uint64_t adims[4] = {(uint64_t)Cin * 2, (uint64_t)W, (uint64_t)H, (uint64_t)B}, astrides[3] = {px, px * W, px * W * H};
+    if ((rc = map_split<F>(&M.a[0], x, 4, adims, astrides, abox, "tc32 activations"))) return rc;
     M.a[1] = M.a[0]; M.a[2] = M.a[0]; M.a[3] = M.a[0];
-    if ((rc = make_w_map<F>(&M.b, weight, (long long)Cin, 8LL * Cout))) return rc;
-    P.H = H; P.W = W; P.ntaps = 1; P.mode = 2; P.n_tiles = 4 * Cout / 64;
+    P.H = H; P.W = W;
+    if (kind == 0) {
+      K = 9LL * Cin;
+      P.ntaps = 9; P.n_tiles = Cout / 64;
+      for (int t = 0; t < 9; ++t) { P.dx[t] = t % 3 - 1; P.dy[t] = t / 3 - 1; }
+    } else {
+      rows = 8LL * Cout;
+      P.ntaps = 1; P.mode = 2; P.n_tiles = 4 * Cout / 64;
+    }
   }
+  const uint64_t wdims[2] = {(uint64_t)K, (uint64_t)rows}, wstride = (uint64_t)K * F::EB;
+  const uint32_t wbox[2] = {2 * F::CH, 128};
+  if ((rc = map_split<F>(&M.b, weight, 2, wdims, &wstride, wbox, "tc32 weights"))) return rc;
   P.tiles_x = ceil_div(P.W, TX); P.tiles_y = ceil_div(P.H, TY);
   // every 2x2 layer gains from sharing the activation tile between its N tiles (down 64 -> 128: 402 -> 297 us, up 256 -> 128: 415 -> 263 us):
   // with the N tile outermost each activation byte crossed HBM n_tiles (2 .. 8) times
   P.ngrp = getenv("DINVK_TC32_NT_OUTER") ? 1 : P.n_tiles;
-  return launch<F>(M, P, stream);
+  return launch_persistent(conv_tc32_kernel<F>, THREADS, SMEM, (long long)P.B * P.tiles_y * P.tiles_x * P.n_tiles, stream, M, P);
 }
 
 template <class F>
@@ -1147,15 +1088,19 @@ static int conv_slab(const void* x, const void* weight, const float* bias, const
   DINVK_CHECK_ARG(Cout % 64 == 0 && Cout >= 64, "conv_tc32_slab: Cout=%d must be a multiple of 64", Cout);
   if (B == 0) return DINVK_OK;
   Maps M;
-  Params P;
+  Params P{};
   int rc;
-  const long long px = (long long)Cin * 2 * F::EB;
-  if ((rc = make_act_map<F>(&M.a[0], x, B, H, W, Cin, px, px * W, px * W * H, slab::SLAB_X, slab::SLAB_Y))) return rc;
+  const uint64_t px = (uint64_t)Cin * 2 * F::EB;
+  const uint64_t adims[4] = {(uint64_t)Cin * 2, (uint64_t)W, (uint64_t)H, (uint64_t)B}, astrides[3] = {px, px * W, px * W * H};
+  const uint32_t abox[4] = {2 * F::CH, slab::SLAB_X, slab::SLAB_Y, 1};
+  if ((rc = map_split<F>(&M.a[0], x, 4, adims, astrides, abox, "tc32 activations"))) return rc;
   M.a[1] = M.a[0]; M.a[2] = M.a[0]; M.a[3] = M.a[0];
-  if ((rc = make_w_map<F>(&M.b, weight, 10LL * Cin, 2LL * Cout))) return rc;
+  const uint64_t wdims[2] = {10ull * Cin, 2ull * Cout}, wstride = 10ull * Cin * F::EB;
+  const uint32_t wbox[2] = {2 * F::CH, 128};
+  if ((rc = map_split<F>(&M.b, weight, 2, wdims, &wstride, wbox, "tc32 weights"))) return rc;
   P.B = B; P.H = H; P.W = W; P.Cin = Cin; P.Cout = Cout;
-  P.ntaps = 9; P.kc_per_tap = Cin / F::CH; P.mode = 0; P.n_tiles = Cout / 64;
-  for (int t = 0; t < 9; ++t) { P.dx[t] = t % 3 - 1; P.dy[t] = t / 3 - 1; P.amap[t] = 0; }
+  P.ntaps = 9; P.kc_per_tap = Cin / F::CH; P.n_tiles = Cout / 64;
+  for (int t = 0; t < 9; ++t) { P.dx[t] = t % 3 - 1; P.dy[t] = t / 3 - 1; }
   P.relu = act; P.res = res; P.res2 = res2; P.out = out; P.bias = bias; P.flag = flag;
   // accumulation window in channel blocks: ONE block by default = 18 full-scale accumulations (tf32: k = 144, fp16: k = 288),
   // so that the tensor core's own fp32 accumulation only ever sees short partial sums (DESIGN §4.4)
@@ -1170,7 +1115,8 @@ static int conv_slab(const void* x, const void* weight, const float* bias, const
     while (g > 1 && P.n_tiles % g) --g;
     P.ngrp = std::max(1, std::min(g, P.n_tiles));
   }
-  return launch_slab<F>(M, P, stream);
+  return launch_persistent(conv_tc32_slab_kernel<F>, slab::THREADS, slab::SMEM_BYTES, (long long)P.B * P.tiles_y * P.tiles_x * P.n_tiles,
+                           stream, M, P);
 }
 
 #endif  // !DINVK_EMUL

@@ -7,40 +7,30 @@
 #ifndef DINVK_EMUL
 #include <cuda.h>
 #include <cuda_runtime.h>
-#include <mutex>
 
+#include "common.cuh"
 #include "tc_ptx.cuh"
 
 namespace dinvk {
+
+// The one tiled tensor-map encoder of the library (cuTensorMapEncodeTiled, resolved from the driver on first use): dims[0] is
+// the contiguous axis, byte_strides holds the rank - 1 outer strides, unit element strides, no interleave, out-of-range
+// elements read as zero.  Returns DINVK_OK, or DINVK_ECUDA with an error message naming `what` (no message when `what` is null).
+int encode_tiled(CUtensorMap* m, CUtensorMapDataType type, int rank, const void* ptr, const uint64_t* dims, const uint64_t* byte_strides,
+                 const uint32_t* box, CUtensorMapSwizzle swizzle, CUtensorMapL2promotion l2, const char* what);
+
 namespace tt {
 
 typedef CUtensorMap TileMap;
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static inline EncodeTiledFn get_encode() {
-  static EncodeTiledFn fn = nullptr;
-  static std::once_flag once;
-  std::call_once(once, []() {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess && qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(p);
-  });
-  return fn;
-}
-
-// true when the geometry can be expressed as a tensor map and the map was built
+// true when the geometry can be expressed as a tensor map and the map was built (false: the caller stages cooperatively)
 static inline bool make_map_f32(TileMap* m, const void* ptr, int W, int H, int N, int box_w, int box_h) {
-  EncodeTiledFn enc = get_encode();
-  if (!enc || (reinterpret_cast<uintptr_t>(ptr) & 15) || (W & 3) || (box_w & 3) || box_w > 256 || box_h > 256 || box_w < 1 || box_h < 1) return false;
-  cuuint64_t dims[3] = {(cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
-  cuuint64_t strides[2] = {(cuuint64_t)W * 4, (cuuint64_t)W * H * 4};
-  cuuint32_t box[3] = {(cuuint32_t)box_w, (cuuint32_t)box_h, 1};
-  cuuint32_t es[3] = {1, 1, 1};
-  return enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<void*>(ptr), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-             CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+  if ((reinterpret_cast<uintptr_t>(ptr) & 15) || (W & 3) || (box_w & 3) || box_w > 256 || box_h > 256 || box_w < 1 || box_h < 1) return false;
+  const uint64_t dims[3] = {(uint64_t)W, (uint64_t)H, (uint64_t)N};
+  const uint64_t strides[2] = {(uint64_t)W * 4, (uint64_t)W * H * 4};
+  const uint32_t box[3] = {(uint32_t)box_w, (uint32_t)box_h, 1};
+  return encode_tiled(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, ptr, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_NONE,
+                      CU_TENSOR_MAP_L2_PROMOTION_L2_128B, nullptr) == DINVK_OK;
 }
 
 __device__ __forceinline__ void tma_load_3d(void* smem, const TileMap* m, uint64_t* bar, int c0, int c1, int c2) {
