@@ -15,13 +15,12 @@
 // Weight layout: per 64-row N tile 128 rows [W_hi (64 couts); W_lo (64 couts)], K-major, k = tap*Cin + c, both parts
 //   rounded to tf32.
 // One MMA "k step" on a 128-byte A row: steps 0,1 = the hi channels, steps 2,3 = the lo channels.
-//   hi step: A_hi x [W_hi; W_lo]  (N = 128)  -> columns [0,64) main, [64,128) corr
-//   lo step: A_lo x  W_hi         (N =  64)  -> columns [64,128) corr
-// With wgmma's register accumulators the corr columns of the N = 128 fragment are exactly the registers of an N = 64
-// fragment (registers 32..63), so the lo steps accumulate into the upper half of the same register array.
+//   hi step: A_hi x W_hi -> main,  A_hi x W_lo -> corr
+//   lo step: A_lo x W_hi -> corr
+// Every product is an N = 64 wgmma on a whole 32-register accumulator array: main = registers 0..31, corr = 32..63.
 //
-// Kernels (persistent, one CTA per SM): consumer warpgroups issue wgmma (M = 64 rows each), drain and run the epilogue
-// from registers; one extra warp is the TMA producer.
+// Kernels (persistent, one CTA per SM): consumer warpgroups issue wgmma (M = 64 rows each), drain, and run the epilogue
+// through a per-warp shared-memory staging buffer; one extra warp (warpgroup) is the TMA producer.
 #include "common.cuh"
 #ifndef DINVK_EMUL
 #include "tc_ptx.cuh"
@@ -48,7 +47,8 @@ constexpr int A_TILE = 128 * 128;          // one 16-channel block of 128 pixels
 constexpr int B_TILE = 128 * 128;          // [W_hi; W_lo] x 32 channels: 16 KB
 constexpr int STAGE = 2 * A_TILE + B_TILE; // two channel blocks of one tap + their weights
 constexpr int STAGES = 4;
-constexpr int SMEM = STAGES * STAGE + 1024;
+constexpr int STG_WARP = 16 * 32;          // epilogue staging buffer of one consumer warp: 16 rows x 32 fp32 columns (2 KB)
+constexpr int SMEM = STAGES * STAGE + 8 * STG_WARP * 4 + 1024;
 constexpr int THREADS = 2 * 128 + 32;      // two consumer warpgroups (GEMM rows [0, 64), [64, 128)) + the TMA producer warp
 
 __device__ __forceinline__ float rna_tf32(float x) {
@@ -87,37 +87,23 @@ struct FmtF16 {
 };
 
 #ifndef DINVK_EMUL
-template <class F, int N>
+template <class F>
 __device__ __forceinline__ void mma(float* d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi, uint32_t accumulate) {
-  if constexpr (F::ID == 0) {
-    if constexpr (N == 128) tc::wgmma_tf32_n128(d, a_lo, a_hi, b_lo, b_hi, accumulate);
-    else tc::wgmma_tf32_n64(d, a_lo, a_hi, b_lo, b_hi, accumulate);
-  } else {
-    if constexpr (N == 128) tc::wgmma_f16_n128(d, a_lo, a_hi, b_lo, b_hi, accumulate);
-    else tc::wgmma_f16_n64(d, a_lo, a_hi, b_lo, b_hi, accumulate);
-  }
+  if constexpr (F::ID == 0) tc::wgmma_tf32_n64(d, a_lo, a_hi, b_lo, b_hi, accumulate);
+  else tc::wgmma_f16_n64(d, a_lo, a_hi, b_lo, b_hi, accumulate);
 }
 // one 128-byte A row block [hi CH | lo CH] (descriptor a) against the weight rows [W_hi; W_lo] at descriptor b (the block's
 // CH channels): acc[0, 32) main += A_hi W_hi, acc[32, 64) corr += A_hi W_lo + A_lo W_hi.  `fresh` = 0 restarts both.
-template <class F>
-__device__ __forceinline__ void mma_block(float* acc, uint32_t a, uint32_t a_hi, uint32_t b, uint32_t b_hi, uint32_t fresh) {
-  mma<F, 128>(acc, a, a_hi, b, b_hi, fresh);             // hi, first half of the block  x [W_hi; W_lo]
-  mma<F, 128>(acc, a + 2, a_hi, b + 2, b_hi, 1u);        // hi, second half
-  mma<F, 64>(acc + 32, a + 4, a_hi, b, b_hi, 1u);        // lo, first half  x W_hi
-  mma<F, 64>(acc + 32, a + 6, a_hi, b + 2, b_hi, 1u);    // lo, second half
-}
-// the same products as mma_block, as six N = 64 wgmmas on the two 32-register halves (main, corr) of acc, so that every
-// wgmma covers a whole accumulator array: ptxas serializes wgmmas when an N = 64 one updates part of an N = 128 one's
-// registers.  Per register the products and their order are those of mma_block.  W_lo is 64 rows (8 KB = 512 descriptor
-// units) after W_hi.
+// Six N = 64 wgmmas, each on a whole 32-register accumulator array (main or corr): ptxas serializes wgmmas when one
+// updates part of another's registers.  W_lo is 64 rows (8 KB = 512 descriptor units) after W_hi.
 template <class F>
 __device__ __forceinline__ void mma_block64(float* acc, uint32_t a, uint32_t a_hi, uint32_t b, uint32_t b_hi, uint32_t fresh) {
-  mma<F, 64>(acc, a, a_hi, b, b_hi, fresh);                  // hi, first half  x W_hi  (main)
-  mma<F, 64>(acc + 32, a, a_hi, b + 512, b_hi, fresh);       // hi, first half  x W_lo  (corr)
-  mma<F, 64>(acc, a + 2, a_hi, b + 2, b_hi, 1u);             // hi, second half x W_hi
-  mma<F, 64>(acc + 32, a + 2, a_hi, b + 514, b_hi, 1u);      // hi, second half x W_lo
-  mma<F, 64>(acc + 32, a + 4, a_hi, b, b_hi, 1u);            // lo, first half  x W_hi
-  mma<F, 64>(acc + 32, a + 6, a_hi, b + 2, b_hi, 1u);        // lo, second half x W_hi
+  mma<F>(acc, a, a_hi, b, b_hi, fresh);                  // hi, first half  x W_hi  (main)
+  mma<F>(acc + 32, a, a_hi, b + 512, b_hi, fresh);       // hi, first half  x W_lo  (corr)
+  mma<F>(acc, a + 2, a_hi, b + 2, b_hi, 1u);             // hi, second half x W_hi
+  mma<F>(acc + 32, a + 2, a_hi, b + 514, b_hi, 1u);      // hi, second half x W_lo
+  mma<F>(acc + 32, a + 4, a_hi, b, b_hi, 1u);            // lo, first half  x W_hi
+  mma<F>(acc + 32, a + 6, a_hi, b + 2, b_hi, 1u);        // lo, second half x W_hi
 }
 // v[i] (row 16 * (warp % 4) + lane / 4 + 8 * ((i >> 1) & 1), column 8 * (i >> 2) + 2 * (lane % 4) + (i & 1)) += main + corr
 template <class F>
@@ -222,62 +208,128 @@ __device__ __forceinline__ void add_split(const typename F::elem* p, float* v) {
 }
 
 #ifndef DINVK_EMUL
-// the same two conversions for one channel pair (c, c + 1), c even, as the wgmma epilogues hold them; p points at the hi
-// element of channel c in its block (the lo element is CH further)
+// the same two conversions for the 16 / EB consecutive channels of one block whose hi words are 16 bytes (tf32: 4, fp16: 8):
+// a += hi + lo given as the raw 16-byte pieces h (hi words) and l (lo words); the store writes one piece each at p (first
+// hi element) and p + CH
 template <class F>
-__device__ __forceinline__ void add_split_pair(const typename F::elem* p, float& a, float& b) {
+__device__ __forceinline__ void add_split16(const uint4& h, const uint4& l, float (&a)[16 / F::EB]) {
   if constexpr (F::ID == 0) {
-    const float2 h = __ldg(reinterpret_cast<const float2*>(p)), l = __ldg(reinterpret_cast<const float2*>(p + F::CH));
-    a += h.x + l.x;
-    b += h.y + l.y;
+    const float* hf = reinterpret_cast<const float*>(&h);
+    const float* lf = reinterpret_cast<const float*>(&l);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) a[i] += hf[i] + lf[i];
   } else {
-    const float2 h = __half22float2(__ldg(reinterpret_cast<const __half2*>(p)));
-    const float2 l = __half22float2(__ldg(reinterpret_cast<const __half2*>(p + F::CH)));
-    a += h.x + l.x * F::CORR;
-    b += h.y + l.y * F::CORR;
+    const __half2* h2 = reinterpret_cast<const __half2*>(&h);
+    const __half2* l2 = reinterpret_cast<const __half2*>(&l);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const float2 hv = __half22float2(h2[i]), lv = __half22float2(l2[i]);
+      a[2 * i] += hv.x + lv.x * F::CORR;
+      a[2 * i + 1] += hv.y + lv.y * F::CORR;
+    }
   }
 }
 template <class F>
-__device__ __forceinline__ bool store_split_pair(typename F::elem* p, float a, float b) {
-  if constexpr (F::ID == 0) {
-    const float ha = rna_tf32(a), hb = rna_tf32(b);
-    *reinterpret_cast<float2*>(p) = make_float2(ha, hb);
-    *reinterpret_cast<float2*>(p + F::CH) = make_float2(a - ha, b - hb);
-    return false;
-  } else {
-    const __half h0 = __float2half_rn(a), h1 = __float2half_rn(b);
-    const __half l0 = __float2half_rn((a - __half2float(h0)) * 2048.0f), l1 = __float2half_rn((b - __half2float(h1)) * 2048.0f);
-    *reinterpret_cast<__half2*>(p) = __halves2half2(h0, h1);
-    *reinterpret_cast<__half2*>(p + F::CH) = __halves2half2(l0, l1);
-    return !(fabsf(a) < 65000.0f) || !(fabsf(b) < 65000.0f);
-  }
-}
-
-// epilogue of the drained sums v (see drain) of one m64 x 64-column block: bias, ReLU, residuals, split store.  The caller
-// maps the thread's two rows to pixels; n0 = first GEMM column of the N tile.
-template <class F>
-__device__ __forceinline__ void epilogue_split(const Params& P, float* v, int b, const int (&y)[2], const int (&x)[2], int n0) {
-  using E = typename F::elem;
-  const int q = threadIdx.x & 3;
-  const int tap = P.mode == 2 ? n0 / P.Cout : 0;
-  const int c0 = n0 - tap * P.Cout;   // output channel of GEMM column n0
+__device__ __forceinline__ bool store_split16(typename F::elem* p, const float (&a)[16 / F::EB]) {
+  uint32_t h[4], l[4];
   bool bad = false;
 #pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    if (!(y[r] < P.H && x[r] < P.W)) continue;
-    long long pix;   // output pixel index
-    if (P.mode == 2) pix = ((long long)b * (2 * P.H) + 2 * y[r] + (tap >> 1)) * (2LL * P.W) + 2 * x[r] + (tap & 1);
-    else pix = ((long long)b * P.H + y[r]) * P.W + x[r];
+  for (int i = 0; i < 4; ++i) {
+    if constexpr (F::ID == 0) {
+      const float hi = rna_tf32(a[i]);
+      h[i] = __float_as_uint(hi);
+      l[i] = __float_as_uint(a[i] - hi);
+    } else {
+      const float a0 = a[2 * i], a1 = a[2 * i + 1];
+      const __half h0 = __float2half_rn(a0), h1 = __float2half_rn(a1);
+      const __half l0 = __float2half_rn((a0 - __half2float(h0)) * 2048.0f), l1 = __float2half_rn((a1 - __half2float(h1)) * 2048.0f);
+      h[i] = (uint32_t)__half_as_ushort(h0) | ((uint32_t)__half_as_ushort(h1) << 16);
+      l[i] = (uint32_t)__half_as_ushort(l0) | ((uint32_t)__half_as_ushort(l1) << 16);
+      bad |= !(fabsf(a0) < 65000.0f) || !(fabsf(a1) < 65000.0f);
+    }
+  }
+  *reinterpret_cast<uint4*>(p) = make_uint4(h[0], h[1], h[2], h[3]);
+  *reinterpret_cast<uint4*>(p + F::CH) = make_uint4(l[0], l[1], l[2], l[3]);
+  return bad;
+}
+
+// float offset of (row r, 16-byte chunk k) in a warp's epilogue staging buffer (STG_WARP floats: 16 rows x 32 columns).  The
+// chunk is XORed with a function of the row so that the fragment writes (8 bytes per lane, rows lane / 4 and lane / 4 + 8)
+// and the row reads of both formats (16 bytes per lane, see epilogue) are free of bank conflicts.
+__device__ __forceinline__ int stg_off(int r, int k) { return 32 * r + 4 * (k ^ ((2 * r & 6) | ((r >> 2) & 1))); }
+
+// epilogue of the drained sums v (see drain) of one m64 x 64-column block, run by each warp on its 16 rows: bias, ReLU,
+// residuals, split store.  The fragment goes through the warp's staging buffer `stg` 32 columns at a time.  Read back, a
+// lane owns the K = 16 / EB consecutive channels whose hi words are one 16-byte piece: fp16, 8 channels of rows lane % 8
+// (+ 8); tf32, 4 channels of rows lane / 8 (+ 4, 8, 12).  Residuals are read and the split words written as those pieces,
+// so that every warp access covers whole 32-byte sectors of the pixels' [hi | lo] rows, instead of 4- or 8-byte words
+// spread over 8 pixel rows.  pixel_of(m) = output pixel of the warp's row m (0..15), or -1 outside the output;
+// c0 = output channel of column 0.
+template <class F, class PixelOf>
+__device__ __forceinline__ void epilogue(const Params& P, const float* v, float* stg, PixelOf pixel_of, int c0) {
+  using E = typename F::elem;
+  constexpr int K = 16 / F::EB, NP = 16 / K;   // channels per lane, rows per lane (one per pass)
+  const int lane = threadIdx.x & 31, q = lane & 3;
+  const int rl = F::ID == 0 ? lane >> 3 : lane & 7;   // the lane's row in pass 0 (rows of pass p: rl + K p)
+  const int cl = F::ID == 0 ? lane & 7 : lane >> 3;   // the lane's channels: K cl .. K cl + K - 1 of the 32 columns
+  long long pix[NP];
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int c = c0 + 8 * j + 2 * q;
-      float a = v[4 * j + 2 * r], bb = v[4 * j + 2 * r + 1];
-      if (P.bias) { a += __ldg(P.bias + c); bb += __ldg(P.bias + c + 1); }
-      if (P.relu) { a = fmaxf(a, 0.f); bb = fmaxf(bb, 0.f); }
-      const long long o = pix * P.Cout * 2 + (c / F::CH) * 2 * F::CH + (c % F::CH);
-      if (P.res) add_split_pair<F>(static_cast<const E*>(P.res) + o, a, bb);
-      if (P.res2) add_split_pair<F>(static_cast<const E*>(P.res2) + o, a, bb);
-      bad |= store_split_pair<F>(static_cast<E*>(P.out) + o, a, bb);
+  for (int p = 0; p < NP; ++p) pix[p] = pixel_of(rl + K * p);
+  bool bad = false;
+#pragma unroll
+  for (int half = 0; half < 2; ++half) {
+    const int c = c0 + 32 * half + K * cl;
+    const long long oc = (c / F::CH) * 2 * F::CH + (c % F::CH);   // element offset of the lane's channels in a pixel row
+    // every global load of this half is issued before the staging round trip, so that their latencies overlap
+    float4 bv[K / 4];
+    uint4 r1[NP][2], r2[NP][2];   // raw [hi, lo] pieces of res and res2
+#pragma unroll
+    for (int k = 0; k < K / 4; ++k) bv[k] = P.bias ? __ldg(reinterpret_cast<const float4*>(P.bias + c) + k) : make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+    for (int p = 0; p < NP; ++p) {
+      r1[p][0] = r1[p][1] = r2[p][0] = r2[p][1] = make_uint4(0u, 0u, 0u, 0u);
+      if (pix[p] < 0) continue;
+      const long long o = pix[p] * P.Cout * 2 + oc;
+      if (P.res) {
+        r1[p][0] = __ldg(reinterpret_cast<const uint4*>(static_cast<const E*>(P.res) + o));
+        r1[p][1] = __ldg(reinterpret_cast<const uint4*>(static_cast<const E*>(P.res) + o + F::CH));
+      }
+      if (P.res2) {
+        r2[p][0] = __ldg(reinterpret_cast<const uint4*>(static_cast<const E*>(P.res2) + o));
+        r2[p][1] = __ldg(reinterpret_cast<const uint4*>(static_cast<const E*>(P.res2) + o + F::CH));
+      }
+    }
+    __syncwarp();
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int i = 4 * (4 * half + j) + 2 * h;
+        *reinterpret_cast<float2*>(stg + stg_off((lane >> 2) + 8 * h, 2 * j + (q >> 1)) + 2 * (q & 1)) = make_float2(v[i], v[i + 1]);
+      }
+    __syncwarp();
+#pragma unroll
+    for (int p = 0; p < NP; ++p) {
+      if (pix[p] < 0) continue;
+      float a[K];
+#pragma unroll
+      for (int k = 0; k < K / 4; ++k) {
+        const float4 s = *reinterpret_cast<const float4*>(stg + stg_off(rl + K * p, K / 4 * cl + k));
+        a[4 * k] = s.x; a[4 * k + 1] = s.y; a[4 * k + 2] = s.z; a[4 * k + 3] = s.w;
+      }
+      if (P.bias) {
+#pragma unroll
+        for (int k = 0; k < K / 4; ++k) {
+          a[4 * k] += bv[k].x; a[4 * k + 1] += bv[k].y; a[4 * k + 2] += bv[k].z; a[4 * k + 3] += bv[k].w;
+        }
+      }
+      if (P.relu) {
+#pragma unroll
+        for (int e = 0; e < K; ++e) a[e] = fmaxf(a[e], 0.f);
+      }
+      if (P.res) add_split16<F>(r1[p][0], r1[p][1], a);
+      if (P.res2) add_split16<F>(r2[p][0], r2[p][1], a);
+      bad |= store_split16<F>(static_cast<E*>(P.out) + pix[p] * P.Cout * 2 + oc, a);
     }
   }
   if (bad && P.flag) atomicOr(P.flag, 1);
@@ -329,17 +381,18 @@ __global__ void __launch_bounds__(THREADS, 1) conv_tc32_kernel(const __grid_cons
     const int wg = warp >> 2;
     constexpr uint32_t HI = tc::desc_hi_sw128(1024);
     const uint32_t smem_lo = tc::smem_u32(smem) >> 4;
-    float acc[64], v[32];
-#pragma unroll
-    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
     int s = 0; uint32_t ph = 0;
     for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
       int pt, nt; tile_index(P, pixel_tiles, t, pt, nt);
       const int b = pt / (P.tiles_y * P.tiles_x), r = pt - b * (P.tiles_y * P.tiles_x);
       const int y0 = (r / P.tiles_x) * TY, x0 = (r % P.tiles_x) * TX;
+      // as in the slab kernel: defined here, the accumulators hold no registers during the epilogue
+      float acc[64], v[32];
+#pragma unroll
+      for (int i = 0; i < 64; ++i) acc[i] = 0.f;
 #pragma unroll
       for (int i = 0; i < 32; ++i) v[i] = 0.f;
-      int in_win = 0, pend = -1;
+      int in_win = 0;
       for (int kb = 0; kb < nk; ++kb) {
         tc::mbar_wait(&full_bar[s], ph);
         const uint32_t a0 = smem_lo + static_cast<uint32_t>(s) * (STAGE >> 4) + static_cast<uint32_t>(wg * (64 * 128 >> 4));
@@ -347,30 +400,28 @@ __global__ void __launch_bounds__(THREADS, 1) conv_tc32_kernel(const __grid_cons
         tc::wgmma_fence();
 #pragma unroll
         for (int jj = 0; jj < 2; ++jj)  // B: second channel block = +64 bytes inside the weight row
-          mma_block<F>(acc, a0 + jj * (A_TILE >> 4), HI, b0 + jj * 4, HI, (jj | in_win) != 0 ? 1u : 0u);
+          mma_block64<F>(acc, a0 + jj * (A_TILE >> 4), HI, b0 + jj * 4, HI, (jj | in_win) != 0 ? 1u : 0u);
         tc::wgmma_commit();
+        // one wait with a compile-time count at a fixed place, the drain's reads after it: a wait chosen by a runtime branch
+        // (wait<1> inside a window, wait<0> at its end) makes ptxas serialize every wgmma of the kernel
+        tc::wgmma_wait<0>();
+        tc::reg_fence<64>(acc);
+        release_stage(&empty_bar[s]);
         if (++in_win == P.win || kb == nk - 1) {
-          tc::wgmma_wait<0>();
-          tc::reg_fence<64>(acc);
-          if (pend >= 0) release_stage(&empty_bar[pend]);
-          release_stage(&empty_bar[s]);
-          pend = -1;
           drain<F>(v, acc);
           in_win = 0;
-        } else {
-          tc::wgmma_wait<1>();
-          if (pend >= 0) release_stage(&empty_bar[pend]);
-          pend = s;
         }
         if (++s == STAGES) { s = 0; ph ^= 1; }
       }
-      int y[2], x[2];
-#pragma unroll
-      for (int rr = 0; rr < 2; ++rr) {
-        const int m = 64 * wg + 16 * (warp & 3) + (lane >> 2) + 8 * rr;
-        y[rr] = y0 + m / TX; x[rr] = x0 + m % TX;
-      }
-      epilogue_split<F>(P, v, b, y, x, nt * 64);
+      const int tap = P.mode == 2 ? nt * 64 / P.Cout : 0;   // 2x up-scatter: the N tile's output sub-pixel
+      const auto pixel_of = [&](int m) -> long long {
+        const int mm = 64 * wg + 16 * (warp & 3) + m;
+        const int y = y0 + mm / TX, x = x0 + mm % TX;
+        if (!(y < P.H && x < P.W)) return -1;
+        if (P.mode == 2) return ((long long)b * (2 * P.H) + 2 * y + (tap >> 1)) * (2LL * P.W) + 2 * x + (tap & 1);
+        return ((long long)b * P.H + y) * P.W + x;
+      };
+      epilogue<F>(P, v, reinterpret_cast<float*>(smem + STAGES * STAGE) + warp * STG_WARP, pixel_of, nt * 64 - tap * P.Cout);
     }
   }
 }
@@ -390,7 +441,7 @@ __global__ void __launch_bounds__(THREADS, 1) conv_tc32_kernel(const __grid_cons
 // Consumer warpgroup g owns y-half g of the tile as TWO m64 blocks (x-halves 0 and 1, 8 x 8 pixels each): 2 x (64
 // accumulator + 32 drain) registers per thread, which a full producer warpgroup makes room for through setmaxnreg.  The MMAs
 // are N = 64 wgmmas (mma_block64), which ptxas keeps in flight back to back.  Every output element sees the same products in
-// the same order, with the same drains, as with one block per warpgroup and mma_block.
+// the same order, with the same drains, as with one block per warpgroup.
 // ---------------------------------------------------------------------------------------------------------------
 namespace slab {
 constexpr int TXP = 16, TYP = 16;                 // CTA pixel tile
@@ -398,8 +449,8 @@ constexpr int SLAB_X = TXP + 8, SLAB_Y = TYP + 2;
 constexpr int SLAB_BYTES = SLAB_X * SLAB_Y * 128;
 constexpr int A_STAGES = 2, B_STAGES = 6;
 constexpr int WT_TILE = 128 * 128;
-constexpr int SMEM_BYTES = A_STAGES * SLAB_BYTES + B_STAGES * WT_TILE + 1024;
 constexpr int CONSUMER_WARPS = 8;                 // two warpgroups
+constexpr int SMEM_BYTES = A_STAGES * SLAB_BYTES + B_STAGES * WT_TILE + CONSUMER_WARPS * STG_WARP * 4 + 1024;
 constexpr int THREADS = 32 * CONSUMER_WARPS + 128; // + the producer warpgroup (one thread issues the TMA loads)
 // registers per thread after setmaxnreg: the launch gives every thread 65536 / 384 = 168; the producer warpgroup returns
 // what the consumers need for 2 x (64 + 32) live accumulator and drain floats (128 x 40 + 256 x 232 <= 65536)
@@ -527,16 +578,16 @@ __global__ void __launch_bounds__(slab::THREADS, 1) conv_tc32_slab_kernel(const 
         if (++sa == A_STAGES) { sa = 0; pha ^= 1; }
         in_win = last_of_win ? 0 : in_win + 1;
       }
-      int y[2], x[2];
+      float* stg = reinterpret_cast<float*>(smem_b + B_STAGES * WT_TILE) + warp * STG_WARP;
 #pragma unroll
-      for (int rr = 0; rr < 2; ++rr) {
-        const int m = 16 * (warp & 3) + (lane >> 2) + 8 * rr;
-        y[rr] = y0 + 8 * wg + (m >> 3); x[rr] = x0 + (m & 7);
+      for (int blk = 0; blk < 2; ++blk) {   // m64 block blk: x-half blk of the warpgroup's y-half
+        const auto pixel_of = [&](int m) -> long long {
+          const int mm = 16 * (warp & 3) + m;
+          const int y = y0 + 8 * wg + (mm >> 3), x = x0 + 8 * blk + (mm & 7);
+          return y < P.H && x < P.W ? ((long long)b * P.H + y) * P.W + x : -1;
+        };
+        epilogue<F>(P, blk ? v1 : v0, stg, pixel_of, nt * 64);
       }
-      epilogue_split<F>(P, v0, b, y, x, nt * 64);
-#pragma unroll
-      for (int rr = 0; rr < 2; ++rr) x[rr] += 8;
-      epilogue_split<F>(P, v1, b, y, x, nt * 64);
     }
   }
 }
@@ -1012,6 +1063,13 @@ static int map_split(CUtensorMap* m, const void* ptr, int rank, const uint64_t* 
   return encode_tiled(m, F::TM, rank, ptr, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, what);
 }
 
+// the epilogue reads bias, res, res2 and writes out in 16-byte pieces
+static bool epilogue_aligned(const float* bias, const void* res, const void* res2, const void* out) {
+  const uintptr_t any = reinterpret_cast<uintptr_t>(bias) | reinterpret_cast<uintptr_t>(res) | reinterpret_cast<uintptr_t>(res2) |
+                        reinterpret_cast<uintptr_t>(out);
+  return (any & 15) == 0;
+}
+
 static int default_window() {
   static int w = -1;
   if (w < 0) {
@@ -1034,6 +1092,7 @@ static int conv_generic(const void* x, const void* weight, const float* bias, co
   DINVK_CHECK_ARG(Cout % 64 == 0 && Cout >= 64, "conv_tc32: Cout=%d must be a multiple of 64", Cout);
   DINVK_CHECK_ARG(kind != 1 || (H % 2 == 0 && W % 2 == 0), "conv_tc32: 2x2 stride-2 needs even H, W");
   DINVK_CHECK_ARG(kind == 0 || (!res && !res2), "conv_tc32: residual inputs are for kind 0 only");
+  DINVK_CHECK_ARG(epilogue_aligned(bias, res, res2, out), "conv_tc32: bias, res, res2 and out must be 16-byte aligned");
   if (B == 0) return DINVK_OK;
   Maps M;
   Params P{};
@@ -1086,6 +1145,7 @@ static int conv_slab(const void* x, const void* weight, const float* bias, const
   DINVK_CHECK_ARG(B >= 0 && H >= 1 && W >= 1, "conv_tc32_slab: bad shape");
   DINVK_CHECK_ARG(Cin % F::CH == 0 && Cin >= F::CH, "conv_tc32_slab: Cin=%d must be a multiple of %d", Cin, F::CH);
   DINVK_CHECK_ARG(Cout % 64 == 0 && Cout >= 64, "conv_tc32_slab: Cout=%d must be a multiple of 64", Cout);
+  DINVK_CHECK_ARG(epilogue_aligned(bias, res, res2, out), "conv_tc32_slab: bias, res, res2 and out must be 16-byte aligned");
   if (B == 0) return DINVK_OK;
   Maps M;
   Params P{};
