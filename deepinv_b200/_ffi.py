@@ -70,6 +70,13 @@ _SIGNATURES = {
     "dinvk_conv_tc32_tail": (c_int, [c_void_p] * 5 + [c_int] * 6 + [c_void_p, c_void_p]),
     "dinvk_split16_to_nchw": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "dinvk_nchw_to_split16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "dinvk_tv_prox": (c_int, [c_void_p] * 6 + [c_int] * 5 + [c_float, C.c_double, C.c_double, c_int, c_int, c_int,
+                                                               c_void_p, c_size_t, c_void_p]),
+    "dinvk_tv_prox_workspace_bytes": (c_size_t, [c_int] * 4),
+    "dinvk_tv_block": (c_int, [C.POINTER(c_int), C.POINTER(c_int)]),
+    "dinvk_tv_stencil": (c_int, [c_int, c_void_p, c_void_p] + [c_int] * 4 + [c_void_p]),
+    "dinvk_tv_fn": (c_int, [c_void_p, c_void_p] + [c_int] * 5 + [c_void_p, c_size_t, c_void_p]),
+    "dinvk_tv_fn_workspace_bytes": (c_size_t, [c_int] * 4),
 }
 
 

@@ -1,0 +1,490 @@
+// tv.cu — total-variation prox (over-relaxed Chambolle-Pock, temporally blocked) and the TV stencils.
+//
+// Replaces
+//   TVDenoiser.forward / TVL1Denoiser         deepinv/models/tv.py:86-151, 238-239
+//   TVDenoiser.nabla / nabla_adjoint          deepinv/models/tv.py:153-218 (2-D)
+//   TVPrior.fn / grad, TVL1Prior.fn           deepinv/optim/prior.py:507-572, 595-611
+//
+// tv_cp_kernel runs up to K Chambolle-Pock iterations per launch.  Each CTA owns a T x T tile of one (b, c) plane and
+// stages the (T + 2K)^2 region around it: y and x2 live in registers (each thread keeps the pixels it owns for the whole
+// launch), the relaxed-primal difference v = 2x - x2 and the dual u2 (one float2 per pixel, the reference's (B,C,H,W,2)
+// layout) live in shared memory.  An iteration needs u2 one pixel up / left of x and v one pixel down / right of u, so the
+// region that is still valid shrinks by one pixel per side per iteration; after K iterations exactly the T x T core is
+// valid and only it is written back.  Every pixel is the same formula on the same inputs whatever T and K are, so the
+// choice of T and K changes no output bit.
+//
+// Every arithmetic step is rounded separately (__fmul_rn / __fadd_rn: no FMA contraction) in the reference's order, so
+// the iterate follows the fp32 torch loop operation by operation.
+#include "common.cuh"
+
+#ifndef DINVK_TV_TILE
+#define DINVK_TV_TILE 56
+#endif
+#ifndef DINVK_TV_BLOCK
+#define DINVK_TV_BLOCK 4
+#endif
+
+#ifdef DINVK_EMUL
+static inline void tv_fence() { __atomic_thread_fence(__ATOMIC_SEQ_CST); }
+template <typename T> static inline T tv_ldcg(const T* p) { return *p; }
+#else
+__device__ __forceinline__ void tv_fence() { __threadfence(); }
+template <typename T> __device__ __forceinline__ T tv_ldcg(const T* p) { return __ldcg(p); }
+#endif
+
+namespace dinvk {
+namespace tv {
+
+constexpr int T = DINVK_TV_TILE;   // owned tile edge
+constexpr int K = DINVK_TV_BLOCK;  // iterations per launch (= halo width)
+constexpr int R = T + 2 * K;       // staged region edge
+constexpr int NT = 512;
+constexpr int PPT = (R * R + NT - 1) / NT;  // region pixels per thread
+constexpr int NW = NT / 32;
+constexpr size_t SMEM = sizeof(float) * 3 * R * R;  // v (R^2) + u2 (2 R^2)
+static_assert(R % 2 == 0, "u2 rows must stay 8-byte aligned");
+
+// control block at the head of the workspace; zeroed by the first launch call of a prox
+struct Ctrl {
+  int ticket;    // CTAs of the current launch that have finished (the last one resets it)
+  int it_done;   // iterations whose result is in state buffer `cur`
+  int cur;       // 0/1: which ping-pong buffer holds the current state
+  int status;    // RUNNING, FINISHED or REPLAY
+  int replay_n;  // REPLAY: iterations to recompute from buffer `cur`
+  int conv_j1;   // 1 + first converging sub-iteration of the converging launch, 0 if the break test never passed
+  int pad[2];
+};
+enum { RUNNING = 0, FINISHED = 1, REPLAY = 2 };
+constexpr size_t CTRL_BYTES = 64;
+
+struct Params {
+  const float* y;
+  float* x2[2];
+  float2* u2[2];
+  const float* lambd;  // (B,)
+  Ctrl* ctrl;
+  double* slots;       // (n_cta, 2K): per-CTA sums of (x_prev - x2)^2 and (x2 + 1e-12)^2 per sub-iteration
+  int C, H, W, tiles_x, tiles_per_plane, n_cta, n_it_max, mode;
+  float crit, tau, one_plus_tau, sigma, rho;
+};
+
+// dual projection: mode 0 isotropic u / max(|u| / lambd, 1) (tv.py:75-82), mode 1 per-component clamp (tv.py:238-239).
+// torch's clamp propagates NaN (fmaxf would not): lambd = 0 and u = 0 gives 0/0 = NaN exactly as the reference does.
+__device__ __forceinline__ float2 dual_proj(float2 t, float l, int mode) {
+  if (mode == 0) {
+    const float n = sqrtf(__fmaf_rn(t.y, t.y, __fmul_rn(t.x, t.x)));  // torch's CPU vector_norm over two elements
+    const float q = n / l;
+    const float d = q != q ? q : fmaxf(q, 1.f);
+    return make_float2(t.x / d, t.y / d);
+  }
+  const float ax = t.x != t.x ? t.x : fminf(fmaxf(t.x, -l), l);
+  const float ay = t.y != t.y ? t.y : fminf(fmaxf(t.y, -l), l);
+  return make_float2(ax, ay);
+}
+
+__device__ __forceinline__ double warp_sum(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+__global__ void __launch_bounds__(NT) tv_cp_kernel(Params p) {
+  __shared__ double red[NW][2 * K];
+  __shared__ int s_last;
+  // Every CTA reads the control block before any CTA of this launch can change it: only the last CTA to finish writes it.
+  Ctrl* ctrl = p.ctrl;
+  const int status = ctrl->status;
+  if (status == FINISHED) return;
+  const bool replay = status == REPLAY;
+  const int it0 = ctrl->it_done;
+  const int n = replay ? ctrl->replay_n : min(K, p.n_it_max - it0);
+  const int in = ctrl->cur, out = in ^ 1;
+  if (n <= 0) return;
+
+  const int tid = threadIdx.x;
+  const int H = p.H, W = p.W;
+  const int plane = blockIdx.x / p.tiles_per_plane, tile = blockIdx.x % p.tiles_per_plane;
+  const int h0 = (tile / p.tiles_x) * T - K, w0 = (tile % p.tiles_x) * T - K;
+  const long long off = (long long)plane * H * W;
+  const float lam = p.lambd[plane / p.C];
+  const float tau = p.tau, opt = p.one_plus_tau, sigma = p.sigma, rho = p.rho;
+  const float* __restrict__ yg = p.y + off;
+  const float* __restrict__ xin = (in ? p.x2[1] : p.x2[0]) + off;  // no dynamic index into the parameter block
+  const float2* __restrict__ uin = (in ? p.u2[1] : p.u2[0]) + off;
+
+  DINVK_DYN_SMEM(float, sm);
+  float* V = sm;                                     // v = 2x - x2 of the current iteration
+  float2* U = reinterpret_cast<float2*>(sm + R * R);  // u2
+
+  float yv[PPT], xv[PPT];
+#pragma unroll
+  for (int i = 0; i < PPT; ++i) {
+    const int idx = tid + i * NT;
+    yv[i] = 0.f;
+    xv[i] = 0.f;
+    if (idx < R * R) {
+      const int gh = h0 + idx / R, gw = w0 + idx % R;
+      float2 u = make_float2(0.f, 0.f);
+      if (gh >= 0 && gh < H && gw >= 0 && gw < W) {
+        const long long g = (long long)gh * W + gw;
+        yv[i] = yg[g];
+        xv[i] = xin[g];
+        u = uin[g];
+      }
+      U[idx] = u;
+    }
+  }
+  __syncthreads();
+
+  double accd[K], accn[K];
+#pragma unroll
+  for (int s = 0; s < K; ++s) {
+    accd[s] = 0.0;
+    accn[s] = 0.0;
+    if (s < n) {
+      // x = prox_tau_fx(x2 - tau nabla_adjoint(u2), y); v = 2x - x2; x2 += rho (x - x2)   (tv.py:131-133, 135)
+      // valid for region rows / columns [s + 1, R - s): reads u2 at [s, R - s)
+      const int lo = s + 1, hi = R - s;
+#pragma unroll
+      for (int i = 0; i < PPT; ++i) {
+        const int idx = tid + i * NT;
+        const int r = idx / R, c = idx % R;
+        const int gh = h0 + r, gw = w0 + c;
+        if (idx < R * R && r >= lo && r < hi && c >= lo && c < hi && gh >= 0 && gh < H && gw >= 0 && gw < W) {
+          // nabla_adjoint in tv.py:202-216 order: vertical component first, then horizontal; each "-= own, += previous"
+          float a = 0.f;
+          if (gh < H - 1) a = __fsub_rn(a, U[idx].x);
+          if (gh > 0) a = __fadd_rn(a, U[idx - R].x);
+          if (gw < W - 1) a = __fsub_rn(a, U[idx].y);
+          if (gw > 0) a = __fadd_rn(a, U[idx - 1].y);
+          const float xo = xv[i];
+          const float xn = __fadd_rn(__fsub_rn(xo, __fmul_rn(tau, a)), __fmul_rn(tau, yv[i])) / opt;
+          V[idx] = __fsub_rn(__fmul_rn(2.f, xn), xo);
+          const float x2n = __fadd_rn(xo, __fmul_rn(rho, __fsub_rn(xn, xo)));
+          xv[i] = x2n;
+          if (r >= K && r < K + T && c >= K && c < K + T) {
+            const float d = __fsub_rn(xo, x2n), e = __fadd_rn(x2n, 1e-12f);
+            accd[s] += (double)d * (double)d;
+            accn[s] += (double)e * (double)e;
+          }
+        }
+      }
+      __syncthreads();
+      // u = prox_sigma_g_conj(u2 + sigma nabla(v), lambd); u2 += rho (u - u2)   (tv.py:134, 136)
+      // valid for [s + 1, R - s - 1): reads v at [s + 1, R - s)
+      const int hi2 = hi - 1;
+#pragma unroll
+      for (int i = 0; i < PPT; ++i) {
+        const int idx = tid + i * NT;
+        const int r = idx / R, c = idx % R;
+        const int gh = h0 + r, gw = w0 + c;
+        if (idx < R * R && r >= lo && r < hi2 && c >= lo && c < hi2 && gh >= 0 && gh < H && gw >= 0 && gw < W) {
+          const float v = V[idx];
+          const float g0 = gh < H - 1 ? __fsub_rn(V[idx + R], v) : 0.f;  // nabla: zero last row / last column
+          const float g1 = gw < W - 1 ? __fsub_rn(V[idx + 1], v) : 0.f;
+          const float2 uo = U[idx];
+          const float2 t = make_float2(__fadd_rn(uo.x, __fmul_rn(sigma, g0)), __fadd_rn(uo.y, __fmul_rn(sigma, g1)));
+          const float2 u = dual_proj(t, lam, p.mode);
+          U[idx] = make_float2(__fadd_rn(uo.x, __fmul_rn(rho, __fsub_rn(u.x, uo.x))),
+                               __fadd_rn(uo.y, __fmul_rn(rho, __fsub_rn(u.y, uo.y))));
+        }
+      }
+      __syncthreads();
+    }
+  }
+
+  // write back the T x T core
+  float* __restrict__ xout = (out ? p.x2[1] : p.x2[0]) + off;
+  float2* __restrict__ uout = (out ? p.u2[1] : p.u2[0]) + off;
+#pragma unroll
+  for (int i = 0; i < PPT; ++i) {
+    const int idx = tid + i * NT;
+    const int r = idx / R, c = idx % R;
+    const int gh = h0 + r, gw = w0 + c;
+    if (idx < R * R && r >= K && r < K + T && c >= K && c < K + T && gh < H && gw < W) {
+      const long long g = (long long)gh * W + gw;
+      xout[g] = xv[i];
+      uout[g] = U[idx];
+    }
+  }
+
+  // this CTA's share of the break test, one slot per CTA (no float atomics: the sums are reproducible run to run)
+  const int lane = tid & 31, warp = tid >> 5;
+#pragma unroll
+  for (int s = 0; s < K; ++s) {
+    const double d = warp_sum(accd[s]), e = warp_sum(accn[s]);
+    if (lane == 0) {
+      red[warp][s] = d;
+      red[warp][K + s] = e;
+    }
+  }
+  __syncthreads();
+  if (tid < 2 * K) {
+    double v = 0.0;
+    for (int w = 0; w < NW; ++w) v += red[w][tid];
+    p.slots[(long long)blockIdx.x * 2 * K + tid] = v;
+  }
+  tv_fence();
+  __syncthreads();
+  if (tid == 0) s_last = atomicAdd(&ctrl->ticket, 1) == p.n_cta - 1;
+  __syncthreads();
+  if (!s_last) return;
+
+  // last CTA: whole-tensor norms per sub-iteration, summed over the slots in CTA order in fp64
+  tv_fence();
+  __shared__ double tot[2 * K];
+  for (int j = 0; j < 2 * K; ++j) {
+    double v = 0.0;
+    for (int c = tid; c < p.n_cta; c += NT) v += tv_ldcg(p.slots + (long long)c * 2 * K + j);
+    v = warp_sum(v);
+    if (lane == 0) red[warp][0] = v;
+    __syncthreads();
+    if (tid == 0) {
+      double t = 0.0;
+      for (int w = 0; w < NW; ++w) t += red[w][0];
+      tot[j] = t;
+    }
+    __syncthreads();
+  }
+  if (tid == 0) {
+    if (replay) {
+      ctrl->it_done = it0 + n;
+      ctrl->cur = out;
+      ctrl->status = FINISHED;
+    } else {
+      // the reference breaks after iteration it (0-based, counted in every call) when it > 1 and
+      // ||x_prev - x2|| / ||x2 + 1e-12|| < crit, in fp32 (tv.py:139-145)
+      int j = -1;
+      for (int s = 0; s < n; ++s) {
+        if (it0 + s < 2) continue;
+        const float rel = (float)sqrt(tot[s]) / (float)sqrt(tot[K + s]);
+        if (rel < p.crit) { j = s; break; }
+      }
+      if (j < 0) {
+        ctrl->it_done = it0 + n;
+        ctrl->cur = out;
+        ctrl->status = it0 + n >= p.n_it_max ? FINISHED : RUNNING;
+      } else if (j == n - 1) {
+        ctrl->it_done = it0 + n;
+        ctrl->cur = out;
+        ctrl->conv_j1 = j + 1;
+        ctrl->status = FINISHED;
+      } else {
+        // converged inside the block: the next launch recomputes j + 1 iterations from this launch's (intact) input
+        ctrl->replay_n = j + 1;
+        ctrl->conv_j1 = j + 1;
+        ctrl->status = REPLAY;
+      }
+    }
+    ctrl->ticket = 0;
+  }
+}
+
+// ---- stencils ------------------------------------------------------------------------------------------------------
+
+__device__ __forceinline__ float2 nabla_at(const float* x, int h, int w, int H, int W) {
+  const float v = x[(long long)h * W + w];
+  return make_float2(h < H - 1 ? __fsub_rn(x[(long long)(h + 1) * W + w], v) : 0.f,
+                     w < W - 1 ? __fsub_rn(x[(long long)h * W + w + 1], v) : 0.f);
+}
+
+// nabla_adjoint in tv.py:202-216 order, g(h, w) -> component
+template <typename G>
+__device__ __forceinline__ float adjoint_at(G g, int h, int w, int H, int W) {
+  float a = 0.f;
+  if (h < H - 1) a = __fsub_rn(a, g(h, w).x);
+  if (h > 0) a = __fadd_rn(a, g(h - 1, w).x);
+  if (w < W - 1) a = __fsub_rn(a, g(h, w).y);
+  if (w > 0) a = __fadd_rn(a, g(h, w - 1).y);
+  return a;
+}
+
+__global__ void __launch_bounds__(256) nabla_kernel(const float* __restrict__ x, float2* __restrict__ g, int H, int W, long long n) {
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const long long plane = i / ((long long)H * W);
+    const int hw = (int)(i - plane * H * W), h = hw / W, w = hw % W;
+    g[i] = nabla_at(x + plane * H * W, h, w, H, W);
+  }
+}
+
+__global__ void __launch_bounds__(256) nabla_adjoint_kernel(const float2* __restrict__ g, float* __restrict__ x, int H, int W, long long n) {
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const long long plane = i / ((long long)H * W);
+    const int hw = (int)(i - plane * H * W), h = hw / W, w = hw % W;
+    const float2* gp = g + plane * H * W;
+    x[i] = adjoint_at([&](int hh, int ww) { return gp[(long long)hh * W + ww]; }, h, w, H, W);
+  }
+}
+
+// TVPrior.grad (prior.py:544-572): nabla_adjoint(Dx / |Dx|), 0 where |Dx| = 0
+__global__ void __launch_bounds__(256) tv_grad_kernel(const float* __restrict__ x, float* __restrict__ out, int H, int W, long long n) {
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const long long plane = i / ((long long)H * W);
+    const int hw = (int)(i - plane * H * W), h = hw / W, w = hw % W;
+    const float* xp = x + plane * H * W;
+    out[i] = adjoint_at([&](int hh, int ww) {
+      const float2 d = nabla_at(xp, hh, ww, H, W);
+      const float nrm = sqrtf(__fmaf_rn(d.y, d.y, __fmul_rn(d.x, d.x)));
+      return nrm > 0.f ? make_float2(d.x / nrm, d.y / nrm) : make_float2(0.f, 0.f);
+    }, h, w, H, W);
+  }
+}
+
+__device__ __forceinline__ double block_sum(double v, double* part) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  v = warp_sum(v);
+  if (lane == 0) part[warp] = v;
+  __syncthreads();
+  double r = 0.0;
+  if (threadIdx.x == 0)
+    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) r += part[w];
+  __syncthreads();
+  return r;  // valid in thread 0
+}
+
+// TVPrior.fn / TVL1Prior.fn (prior.py:507-522, 595-611), two deterministic stages like dinvk_batched_dot:
+// partial[b, chunk] = sum over the chunk of |Dx| (mode 0: 2-norm over the two differences, mode 1: 1-norm)
+__global__ void __launch_bounds__(256) tv_fn_partial_kernel(double* __restrict__ partial, const float* __restrict__ x, int mode,
+                                                            int C, int H, int W, int chunks) {
+  __shared__ double part[8];
+  const int b = blockIdx.y, ch = blockIdx.x;
+  const long long n_per = (long long)C * H * W;
+  double acc = 0.0;
+  for (long long i = (long long)ch * blockDim.x + threadIdx.x; i < n_per; i += (long long)chunks * blockDim.x) {
+    const int c = (int)(i / ((long long)H * W));
+    const int hw = (int)(i - (long long)c * H * W);
+    const float2 d = nabla_at(x + (long long)b * n_per + (long long)c * H * W, hw / W, hw % W, H, W);
+    acc += mode == 0 ? (double)sqrtf(__fadd_rn(__fmul_rn(d.x, d.x), __fmul_rn(d.y, d.y))) : (double)fabsf(d.x) + (double)fabsf(d.y);
+  }
+  const double r = block_sum(acc, part);
+  if (threadIdx.x == 0) partial[(long long)b * chunks + ch] = r;
+}
+
+__global__ void __launch_bounds__(256) tv_fn_final_kernel(float* __restrict__ out, const double* __restrict__ partial, int chunks) {
+  __shared__ double part[8];
+  const int b = blockIdx.x;
+  double acc = 0.0;
+  for (int i = threadIdx.x; i < chunks; i += blockDim.x) acc += partial[(long long)b * chunks + i];
+  const double r = block_sum(acc, part);
+  if (threadIdx.x == 0) out[b] = (float)r;
+}
+
+static int stencil_grid(long long n) {
+  long long blocks = (n + 255) / 256;
+  const long long cap = (long long)sm_count() * 8;
+  return (int)std::max(1LL, std::min(blocks, cap));
+}
+
+static int fn_chunks(int B, long long n_per) {
+  long long want = (n_per + 256 * 16 - 1) / (256 * 16);
+  const long long cap = std::max(1, sm_count() * 8 / std::max(1, B));
+  return (int)std::max(1LL, std::min(want, cap));
+}
+
+static int tiles(int n) { return (n + T - 1) / T; }
+
+}  // namespace tv
+}  // namespace dinvk
+
+using namespace dinvk;
+
+extern "C" int dinvk_tv_block(int* tile, int* iters) {
+  if (tile) *tile = tv::T;
+  if (iters) *iters = tv::K;
+  return DINVK_OK;
+}
+
+extern "C" size_t dinvk_tv_prox_workspace_bytes(int B, int C, int H, int W) {
+  const size_t n_cta = (size_t)std::max(B, 0) * std::max(C, 0) * tv::tiles(std::max(H, 1)) * tv::tiles(std::max(W, 1));
+  return tv::CTRL_BYTES + sizeof(double) * 2 * tv::K * std::max<size_t>(n_cta, 1);
+}
+
+extern "C" int dinvk_tv_prox(const float* y, float* x2_a, float* u2_a, float* x2_b, float* u2_b, const float* lambd, int B, int C,
+                             int H, int W, int n_it_max, float crit, double tau, double rho, int mode, int first, int n_launch,
+                             void* workspace, size_t workspace_bytes, void* stream) {
+  DINVK_CHECK_ARG(y && x2_a && u2_a && x2_b && u2_b && lambd && workspace, "dinvk_tv_prox: null pointer");
+  DINVK_CHECK_ARG(B >= 0 && C >= 0 && H > 0 && W > 0 && n_it_max >= 0 && n_launch >= 0, "dinvk_tv_prox: bad shape");
+  DINVK_CHECK_ARG(mode == 0 || mode == 1, "dinvk_tv_prox: mode must be 0 (TV) or 1 (TV-L1)");
+  DINVK_CHECK_ARG((reinterpret_cast<uintptr_t>(u2_a) & 7) == 0 && (reinterpret_cast<uintptr_t>(u2_b) & 7) == 0 &&
+                      (reinterpret_cast<uintptr_t>(workspace) & 7) == 0,
+                  "dinvk_tv_prox: u2 buffers and workspace must be 8-byte aligned");
+  if (workspace_bytes < dinvk_tv_prox_workspace_bytes(B, C, H, W))
+    return set_error(DINVK_EWORKSPACE, "dinvk_tv_prox: workspace too small");
+  const long long n_cta = (long long)B * C * tv::tiles(H) * tv::tiles(W);
+  DINVK_CHECK_ARG(n_cta < (1LL << 31), "dinvk_tv_prox: too many tiles");
+  tv::Params p;
+  p.y = y;
+  p.x2[0] = x2_a;
+  p.x2[1] = x2_b;
+  p.u2[0] = reinterpret_cast<float2*>(u2_a);
+  p.u2[1] = reinterpret_cast<float2*>(u2_b);
+  p.lambd = lambd;
+  p.ctrl = reinterpret_cast<tv::Ctrl*>(workspace);
+  p.slots = reinterpret_cast<double*>(static_cast<char*>(workspace) + tv::CTRL_BYTES);
+  p.C = C;
+  p.H = H;
+  p.W = W;
+  p.tiles_x = tv::tiles(W);
+  p.tiles_per_plane = tv::tiles(H) * tv::tiles(W);
+  p.n_cta = (int)n_cta;
+  p.n_it_max = n_it_max;
+  p.mode = mode;
+  p.crit = crit;
+  // the reference's constants: python doubles rounded once to fp32 by torch (tv.py:119-121, 72)
+  p.tau = (float)tau;
+  p.one_plus_tau = (float)(1.0 + tau);
+  p.sigma = (float)(1.0 / tau / 8.0);  // 1 / tau / 2^(ndim - 1) with ndim = 4 (tv.py:119-121)
+  p.rho = (float)rho;
+  if (first) {
+    cudaError_t e = cudaMemsetAsync(workspace, 0, tv::CTRL_BYTES, (cudaStream_t)stream);
+    if (e != cudaSuccess) return set_error(DINVK_ECUDA, "dinvk_tv_prox: memset: %s", cudaGetErrorString(e));
+  }
+  if (n_cta == 0) return DINVK_OK;
+  int rc;
+#ifndef DINVK_EMUL
+  // opt in even at exactly 48 KB of dynamic shared memory: the static reduction buffers come on top of it
+  if ((rc = raise_smem_limit(reinterpret_cast<const void*>(tv::tv_cp_kernel), tv::SMEM))) return rc;
+#endif
+  for (int l = 0; l < n_launch; ++l) {
+    DINVK_LAUNCH(tv::tv_cp_kernel, dim3((unsigned)n_cta), dim3(tv::NT), tv::SMEM, stream, p);
+    if ((rc = DINVK_POST_LAUNCH())) return rc;
+  }
+  return DINVK_OK;
+}
+
+extern "C" int dinvk_tv_stencil(int op, const float* in, float* out, int B, int C, int H, int W, void* stream) {
+  DINVK_CHECK_ARG(in && out && B >= 0 && C >= 0 && H > 0 && W > 0, "dinvk_tv_stencil: bad arguments");
+  DINVK_CHECK_ARG(op >= 0 && op <= 2, "dinvk_tv_stencil: op must be 0 (nabla), 1 (nabla_adjoint) or 2 (TV subgradient)");
+  const long long n = (long long)B * C * H * W;
+  if (n == 0) return DINVK_OK;
+  const dim3 grid(tv::stencil_grid(n));
+  if (op == 0)
+    DINVK_LAUNCH(tv::nabla_kernel, grid, dim3(256), 0, stream, in, reinterpret_cast<float2*>(out), H, W, n);
+  else if (op == 1)
+    DINVK_LAUNCH(tv::nabla_adjoint_kernel, grid, dim3(256), 0, stream, reinterpret_cast<const float2*>(in), out, H, W, n);
+  else
+    DINVK_LAUNCH(tv::tv_grad_kernel, grid, dim3(256), 0, stream, in, out, H, W, n);
+  return DINVK_POST_LAUNCH();
+}
+
+extern "C" size_t dinvk_tv_fn_workspace_bytes(int B, int C, int H, int W) {
+  const long long n_per = (long long)std::max(C, 0) * std::max(H, 0) * std::max(W, 0);
+  return sizeof(double) * (size_t)std::max(1, B) * (size_t)tv::fn_chunks(B, n_per) + 64;
+}
+
+extern "C" int dinvk_tv_fn(float* out, const float* x, int mode, int B, int C, int H, int W, void* workspace, size_t workspace_bytes,
+                           void* stream) {
+  DINVK_CHECK_ARG(out && x && workspace && B >= 0 && C >= 0 && H > 0 && W > 0, "dinvk_tv_fn: bad arguments");
+  DINVK_CHECK_ARG(mode == 0 || mode == 1, "dinvk_tv_fn: mode must be 0 (TV) or 1 (TV-L1)");
+  DINVK_CHECK_ARG(B <= 65535, "dinvk_tv_fn: batch too large");
+  if (B == 0) return DINVK_OK;
+  if (workspace_bytes < dinvk_tv_fn_workspace_bytes(B, C, H, W)) return set_error(DINVK_EWORKSPACE, "dinvk_tv_fn: workspace too small");
+  const int chunks = tv::fn_chunks(B, (long long)C * H * W);
+  double* partial = reinterpret_cast<double*>(((uintptr_t)workspace + 7) & ~(uintptr_t)7);
+  DINVK_LAUNCH(tv::tv_fn_partial_kernel, dim3(chunks, B), dim3(256), 0, stream, partial, x, mode, C, H, W, chunks);
+  DINVK_LAUNCH(tv::tv_fn_final_kernel, dim3(B), dim3(256), 0, stream, out, (const double*)partial, chunks);
+  return DINVK_POST_LAUNCH();
+}

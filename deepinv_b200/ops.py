@@ -586,3 +586,140 @@ def interleaved_to_planar(z: torch.Tensor) -> torch.Tensor:
     if B and n:
         check(get_lib().dinvk_interleaved_to_planar(_p(torch.view_as_real(z)), _p(out), B, n, _stream(dev)))
     return out
+
+
+# --------------------------------------------------------------------------------------------
+# total variation (deepinv/models/tv.py, deepinv/optim/prior.py:485-611)
+# --------------------------------------------------------------------------------------------
+TV_CTRL_FIELDS = ("ticket", "it_done", "cur", "status", "replay_n", "conv_j1")
+TV_RUNNING, TV_FINISHED, TV_REPLAY = 0, 1, 2
+
+
+def tv_block(lib=None) -> tuple[int, int]:
+    """(T, K): the tile edge and the iterations per launch libdinvk's TV prox was compiled with"""
+    t, k = ctypes.c_int(0), ctypes.c_int(0)
+    check((lib or get_lib()).dinvk_tv_block(ctypes.byref(t), ctypes.byref(k)))
+    return t.value, k.value
+
+
+def tv_drive(launch, read_ctrl, n_it_max: int, iters_per_launch: int, check_every: int) -> dict:
+    """Host loop of the TV prox, shared with the emulation tests.
+
+    `launch(first, n)` enqueues n iteration blocks; `read_ctrl()` synchronises and returns the control block as a dict.
+    Issues ceil(n_it_max / K) blocks, reading the control block every `check_every` launches and after the last one;
+    a launch issued after convergence returns at entry.  If the break test passed inside a block, one more launch
+    replays the iterations up to the break.  Returns the final control block plus the launch and synchronisation counts.
+    """
+    total = -(-int(n_it_max) // iters_per_launch)
+    issued = syncs = 0
+    ctrl = {"it_done": 0, "cur": 0, "status": TV_FINISHED, "conv_j1": 0}
+    while issued < total:
+        k = min(max(1, int(check_every)), total - issued)
+        launch(issued == 0, k)
+        issued += k
+        ctrl = read_ctrl()
+        syncs += 1
+        if ctrl["status"] != TV_RUNNING:
+            break
+    if ctrl["status"] == TV_REPLAY:
+        launch(False, 1)
+        issued += 1
+        ctrl = dict(ctrl, cur=ctrl["cur"] ^ 1, it_done=ctrl["it_done"] + ctrl["replay_n"], status=TV_FINISHED)
+    ctrl.update(launches=issued, syncs=syncs)
+    return ctrl
+
+
+def tv_prox(y: torch.Tensor, lambd: torch.Tensor, x2: torch.Tensor, u2: torch.Tensor, l1: bool = False, tau: float = 0.01,
+            rho: float = 1.99, n_it_max: int = 1000, crit: float = 1e-5, check_every: int = 16, stats: Optional[dict] = None):
+    """TVDenoiser / TVL1Denoiser iterations from the state (x2 (B,C,H,W), u2 (B,C,H,W,2)); lambd (B,) on the device.
+
+    Returns (x2, u2, iterations) with the iteration count as a 0-d int32 device tensor.  `stats`, if given, receives the
+    launch and host-synchronisation counts of this call.
+    """
+    dev = _require_cuda(y, lambd, x2, u2)
+    if y.dim() != 4:
+        raise NotImplementedError(f"the TV prox is 2-D only: expected (B, C, H, W), got {tuple(y.shape)}")
+    y, lambd = _f32c(y), _f32c(lambd)
+    B, C, H, W = y.shape
+    if lambd.numel() != B:
+        raise DinvkError(f"lambd must hold one value per sample: {lambd.numel()} values for a batch of {B}")
+    # ping-pong state buffers: (a) the start state, (b) scratch; a replay needs its launch's input intact
+    xa, ua = x2.float().clone(memory_format=torch.contiguous_format), u2.float().clone(memory_format=torch.contiguous_format)
+    xb, ub = torch.empty_like(xa), torch.empty_like(ua)
+    lib = get_lib()
+    nb = lib.dinvk_tv_prox_workspace_bytes(B, C, H, W)
+    ws = torch.empty(nb, dtype=torch.uint8, device=dev)  # per call: the control block is the solve's state
+    stream = _stream(dev)
+    _, K = tv_block(lib)
+
+    def launch(first, n):
+        check(lib.dinvk_tv_prox(_p(y), _p(xa), _p(ua), _p(xb), _p(ub), _p(lambd), B, C, H, W, int(n_it_max), float(crit),
+                                float(tau), float(rho), int(l1), int(first), n, _p(ws), nb, stream))
+
+    def read_ctrl():
+        return dict(zip(TV_CTRL_FIELDS, ws[:24].view(torch.int32).tolist()))
+
+    if n_it_max <= 0 or y.numel() == 0:
+        ctrl = {"cur": 0, "launches": 0, "syncs": 0}
+        iters = torch.zeros((), dtype=torch.int32, device=dev)
+    else:
+        ctrl = tv_drive(launch, read_ctrl, n_it_max, K, check_every)
+        iters = torch.full((), ctrl["it_done"], dtype=torch.int32, device=dev)
+    if stats is not None:
+        stats.update(launches=ctrl["launches"], syncs=ctrl["syncs"], converged=bool(ctrl.get("conv_j1", 0)))
+    return (xb, ub, iters) if ctrl["cur"] else (xa, ua, iters)
+
+
+def _tv_shape(x: torch.Tensor, what: str) -> None:
+    if x.dim() != 4:
+        raise NotImplementedError(f"{what} is 2-D only: expected a (B, C, H, W) tensor, got {tuple(x.shape)}")
+
+
+def tv_nabla(x: torch.Tensor) -> torch.Tensor:
+    """finite differences (B,C,H,W) -> (B,C,H,W,2) (tv.py:153-181)"""
+    dev = _require_cuda(x)
+    _tv_shape(x, "nabla")
+    x = _f32c(x)
+    out = torch.empty((*x.shape, 2), dtype=torch.float32, device=dev)
+    if x.numel():
+        check(get_lib().dinvk_tv_stencil(0, _p(x), _p(out), *x.shape, _stream(dev)))
+    return out
+
+
+def tv_nabla_adjoint(g: torch.Tensor) -> torch.Tensor:
+    """adjoint of the finite differences (B,C,H,W,2) -> (B,C,H,W) (tv.py:183-218)"""
+    dev = _require_cuda(g)
+    if g.dim() != 5 or g.shape[-1] != 2:
+        raise NotImplementedError(f"nabla_adjoint is 2-D only: expected a (B, C, H, W, 2) tensor, got {tuple(g.shape)}")
+    g = _f32c(g)
+    out = torch.empty(g.shape[:-1], dtype=torch.float32, device=dev)
+    if g.numel():
+        check(get_lib().dinvk_tv_stencil(1, _p(g), _p(out), *g.shape[:-1], _stream(dev)))
+    return out
+
+
+def tv_grad(x: torch.Tensor) -> torch.Tensor:
+    """TV subgradient nabla_adjoint(Dx / |Dx|), 0 where |Dx| = 0 (prior.py:544-572)"""
+    dev = _require_cuda(x)
+    _tv_shape(x, "TVPrior.grad")
+    x = _f32c(x)
+    out = torch.empty_like(x)
+    if x.numel():
+        check(get_lib().dinvk_tv_stencil(2, _p(x), _p(out), *x.shape, _stream(dev)))
+    return out
+
+
+def tv_fn(x: torch.Tensor, l1: bool = False) -> torch.Tensor:
+    """(B,) TV value: sum of |Dx| with the 2-norm (TVPrior.fn) or 1-norm (TVL1Prior.fn) over the differences"""
+    dev = _require_cuda(x)
+    _tv_shape(x, "TVPrior.fn")
+    x = _f32c(x)
+    B, C, H, W = x.shape
+    out = torch.zeros(B, dtype=torch.float32, device=dev)
+    if x.numel() == 0:
+        return out
+    lib = get_lib()
+    nb = lib.dinvk_tv_fn_workspace_bytes(B, C, H, W)
+    ws = workspace(dev, nb, "tv_fn")
+    check(lib.dinvk_tv_fn(_p(out), _p(x), int(l1), B, C, H, W, _p(ws), ws.numel(), _stream(dev)))
+    return out

@@ -8,4 +8,4 @@ from .optimizers import (ADMM, DRS, FISTA, GD, HQS, PDCP, PGD, AndersonAccelerat
                          DEQConfig,  # noqa: F401
                          create_iterator,
                          optim_builder)
-from .prior import RED, PnP, Prior, Tikhonov, ZeroPrior  # noqa: F401
+from .prior import RED, PnP, Prior, Tikhonov, TVL1Prior, TVPrior, ZeroPrior  # noqa: F401

@@ -89,3 +89,43 @@ class Tikhonov(Prior):
 
     def prox(self, x, *args, gamma=1.0, **kwargs):
         return (1 / (gamma + 1)) * x
+
+
+class TVPrior(Prior):
+    """Total variation g(x) = ||Dx||_{1,2} (prior.py:485-572).  prox = TVDenoiser(x, ths=gamma) with crit=def_crit; fn, grad,
+    nabla and nabla_adjoint are one libdinvk launch each (fn: two).  prox_conjugate comes from Prior (Moreau), so PDCP runs."""
+
+    _l1 = False
+
+    def __init__(self, def_crit=1e-8, n_it_max=1000, *args, **kwargs):
+        super().__init__(*args, **kwargs)
+        self.explicit_prior = True
+        from ..models.tv import TVDenoiser, TVL1Denoiser
+
+        self.TVModel = (TVL1Denoiser if self._l1 else TVDenoiser)(crit=def_crit, n_it_max=n_it_max)
+
+    def fn(self, x, *args, **kwargs):
+        from .. import ops
+
+        return ops.tv_fn(x, l1=self._l1)
+
+    def prox(self, x, *args, gamma=1.0, **kwargs):
+        return self.TVModel(x, ths=gamma)
+
+    def nabla(self, x):
+        return self.TVModel.nabla(x)
+
+    def nabla_adjoint(self, x):
+        return self.TVModel.nabla_adjoint(x)
+
+    def grad(self, x, *args, **kwargs):
+        """subgradient -div(Dx / |Dx|), the zero element where Dx = 0 (prior.py:544-572)"""
+        from .. import ops
+
+        return ops.tv_grad(x)
+
+
+class TVL1Prior(TVPrior):
+    """g(x) = ||Dx||_1 (prior.py:575-611); prox by TVL1Denoiser, grad inherited from TVPrior as in the reference"""
+
+    _l1 = True

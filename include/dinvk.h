@@ -312,6 +312,39 @@ int dinvk_conv_tc32_tail(const void* x, const float* weight, const float* bias, 
 int dinvk_split16_to_nchw(const void* in, float* out, int B, int C, int H, int W, int fmt, void* stream);
 int dinvk_nchw_to_split16(const float* in, void* out, int B, int C, int H, int W, int fmt, void* stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Total variation (2-D, images (B,C,H,W) fp32; gradient fields (B,C,H,W,2), component 0 vertical)
+ * ------------------------------------------------------------------------------------------
+ * TV prox by over-relaxed Chambolle-Pock, TVDenoiser.forward / TVL1Denoiser (deepinv/models/tv.py:86-151, 238-239).
+ * Each launch runs up to `dinvk_tv_block` iterations of tv.py:131-137 on two ping-pong state buffers
+ * (x2_a, u2_a) / (x2_b, u2_b), reads the per-sample lambd (B,) from device memory and applies the reference's break
+ * test (it > 1 and ||x_prev - x2|| / ||x2 + 1e-12|| < crit over the whole tensor, tv.py:139-145) for every iteration
+ * without a host synchronisation.  The state of the solve lives in a 64-byte control block at the head of the workspace,
+ * int32 [ticket, it_done, cur, status, replay_n, conv_j1, -, -]:
+ *   it_done  iterations whose result is in buffer `cur` (0: a, 1: b);  status 0 running, 1 finished, 2 replay pending;
+ *   conv_j1  1 + the sub-iteration of the converging launch at which the test passed (0: it never passed).
+ * If the test passes before the last iteration of a launch, the next launch recomputes the iterations up to the break
+ * from that launch's input into its output (status 2), so the result is bitwise the state after the reference's break
+ * iteration.  Launches issued after the solve finished return at entry.  first != 0 zeroes the control block (call it
+ * that way once per prox, with (x2_a, u2_a) holding the start state); each call enqueues n_launch launches.
+ * mode 0: isotropic dual projection u / max(|u| / lambd, 1) (TV), 1: per-component clamp to [-lambd, lambd] (TV-L1).
+ * tau, rho: the reference's python floats; sigma = 1 / tau / 8 and 1 + tau are formed in double and rounded once. */
+int dinvk_tv_prox(const float* y, float* x2_a, float* u2_a, float* x2_b, float* u2_b, const float* lambd, int B, int C,
+                  int H, int W, int n_it_max, float crit, double tau, double rho, int mode, int first, int n_launch,
+                  void* workspace, size_t workspace_bytes, void* stream);
+size_t dinvk_tv_prox_workspace_bytes(int B, int C, int H, int W);
+/* the library's compile-time tile edge T and iterations per launch K of dinvk_tv_prox (host pointers) */
+int dinvk_tv_block(int* tile_host, int* iters_host);
+/* one-launch stencils: op 0 nabla (tv.py:153-181) in (B,C,H,W) -> out (B,C,H,W,2); op 1 nabla_adjoint (tv.py:183-218)
+ * (B,C,H,W,2) -> (B,C,H,W); op 2 the TV subgradient nabla_adjoint(Dx / |Dx|), 0 where |Dx| = 0 (TVPrior.grad,
+ * deepinv/optim/prior.py:544-572) */
+int dinvk_tv_stencil(int op, const float* in, float* out, int B, int C, int H, int W, void* stream);
+/* per-sample TV value (TVPrior.fn / TVL1Prior.fn, prior.py:507-522, 595-611): out[b] = sum |Dx| with the 2-norm over
+ * the two differences (mode 0) or the 1-norm (mode 1); fp64 across the block and the chunks, deterministic */
+int dinvk_tv_fn(float* out, const float* x, int mode, int B, int C, int H, int W, void* workspace,
+                size_t workspace_bytes, void* stream);
+size_t dinvk_tv_fn_workspace_bytes(int B, int C, int H, int W);
+
 #ifdef __cplusplus
 }
 #endif
