@@ -17,6 +17,10 @@
 //                              transpose of the padding folds the border strips back (fold kernel).
 // A CTA computes a 64x64 output tile; each thread owns 4x4 outputs and slides a 4-wide register window
 // along the filter row (one 128-bit shared load per 16 FMAs per row).  Filters up to ~128x128 fit.
+//
+// The space-varying blur (product convolution, SpaceVaryingBlur) runs the same tile and window loop K times per CTA, once per
+// term, into one set of accumulators: svblur_fwd_kernel on the product patch w_k . x, svblur_adj_kernel on the y patch with a
+// per-pixel multiplier applied to each term's partial block.  The replicate / reflect adjoint folds once, after the K terms.
 #include "common.cuh"
 #include "tma_tile.cuh"
 
@@ -42,6 +46,98 @@ __device__ __forceinline__ int map_index(int a, int n, int mode, bool& ok) {
   if (mode == 3) { if (a < 0) a = -a; if (a > n - 1) a = 2 * (n - 1) - a; ok = (a >= 0 && a < n); return ok ? a : 0; }
   ok = (a >= 0 && a < n);
   return ok ? a : 0;
+}
+
+// Helpers of the space-varying kernels below: the staging and window loop of blur_corr_kernel, factored out.  blur_corr_kernel
+// keeps its own inline copy so that its code generation stays exactly as it was.
+//
+// the filter of one term, staged as the window loop reads it: ks[u][v] for v < wp, `shift` leading zero taps (see corr_params)
+__device__ __forceinline__ void stage_filter(float* ks, const float* __restrict__ f, const BlurParams& P) {
+  for (int idx = threadIdx.x; idx < P.h * P.wp; idx += 256) {
+    const int u = idx / P.wp, v = idx - u * P.wp - P.shift;
+    float val = 0.f;
+    if (v >= 0 && v < P.w) val = P.flip ? __ldg(f + (P.h - 1 - u) * P.w + (P.w - 1 - v)) : __ldg(f + u * P.w + v);
+    ks[idx] = val;
+  }
+}
+
+// The input tile + halo of plane `bc`, rows i0 + off_i.., columns j0 + off_j...  Zero padding (and every tile whose halo stays inside
+// the image, whatever the padding rule) is ONE tensor-map box load: the copy engine zero-fills out-of-range elements.  Tiles that
+// touch the border under circular / replicate / reflect padding resolve the rule in index space with the cooperative loop.
+// No barrier at the end: the caller's __syncthreads publishes the patch.
+__device__ __forceinline__ void stage_patch(float* patch, const tt::TileMap* tmap, int use_tma, const float* __restrict__ src,
+                                            const BlurParams& P, int i0, int j0, int bc) {
+  const int PH = BL_T + P.h - 1;
+  bool by_tma = false;
+#ifndef DINVK_EMUL
+  if (use_tma) {
+    const int r0 = i0 + P.off_i, c0 = j0 + P.off_j;
+    by_tma = (P.map == 0) || (r0 >= 0 && r0 + PH <= P.Hin && c0 >= 0 && c0 + P.PW <= P.Win);
+    if (by_tma) {   // (uniform over the CTA)
+      __shared__ __align__(8) uint64_t tile_bar;
+      tt::stage_tile(patch, tmap, &tile_bar, c0, r0, bc, (uint32_t)(PH * P.PW * 4));
+    }
+  }
+#else
+  (void)tmap; (void)use_tma; (void)bc;
+#endif
+  if (!by_tma) {
+    for (int idx = threadIdx.x; idx < PH * P.PW; idx += 256) {
+      const int pr = idx / P.PW, pc = idx - pr * P.PW;
+      bool okr, okc;
+      const int gi = map_index(i0 + pr + P.off_i, P.Hin, P.map, okr);
+      const int gj = map_index(j0 + pc + P.off_j, P.Win, P.map, okc);
+      patch[idx] = (okr && okc) ? __ldg(src + (long long)gi * P.Win + gj) : 0.f;
+    }
+  }
+}
+
+// the 4x4 register-tiled sliding window: acc[r][q] += sum_{u,v} ks[u][v] * patch[ty*4 + r + u][tx*4 + q + v], one 128-bit shared
+// load per 16 FMAs per filter row
+__device__ __forceinline__ void window_fma(const float* patch, const float* ks, const BlurParams& P, int tx, int ty, float (&acc)[4][4]) {
+  const int nchunk = P.wp >> 2;
+  for (int u = 0; u < P.h; ++u) {
+    float4 lo[4];
+#pragma unroll
+    for (int r = 0; r < 4; ++r) lo[r] = *reinterpret_cast<const float4*>(&patch[(ty * 4 + r + u) * P.PW + tx * 4]);
+    const float4* krow = reinterpret_cast<const float4*>(&ks[u * P.wp]);
+    for (int vb = 0; vb < nchunk; ++vb) {
+      const float4 k4 = krow[vb];
+#pragma unroll
+      for (int r = 0; r < 4; ++r) {
+        const float4 hi = *reinterpret_cast<const float4*>(&patch[(ty * 4 + r + u) * P.PW + tx * 4 + 4 * vb + 4]);
+        const float win[8] = {lo[r].x, lo[r].y, lo[r].z, lo[r].w, hi.x, hi.y, hi.z, hi.w};
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          float a = acc[r][q];
+          a = fmaf(k4.x, win[q], a);
+          a = fmaf(k4.y, win[q + 1], a);
+          a = fmaf(k4.z, win[q + 2], a);
+          a = fmaf(k4.w, win[q + 3], a);
+          acc[r][q] = a;
+        }
+        lo[r] = hi;
+      }
+    }
+  }
+}
+
+__device__ __forceinline__ float* align128(float* p) {
+  return reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(p) + 127) & ~static_cast<uintptr_t>(127));
+}
+
+__device__ __forceinline__ void store_tile(float* __restrict__ dst, const float (&acc)[4][4], const BlurParams& P, int i0, int j0,
+                                           int tx, int ty) {
+#pragma unroll
+  for (int r = 0; r < 4; ++r) {
+    const int gi = i0 + ty * 4 + r;
+    if (gi >= P.Hout) continue;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const int gj = j0 + tx * 4 + q;
+      if (gj < P.Wout) dst[(long long)gi * P.Wout + gj] = acc[r][q];
+    }
+  }
 }
 
 __global__ void __launch_bounds__(256) blur_corr_kernel(const __grid_constant__ tt::TileMap tmap, int use_tma,
@@ -133,6 +229,117 @@ __global__ void __launch_bounds__(256) blur_corr_kernel(const __grid_constant__ 
   }
 }
 
+// ---- space-varying blur (product convolution) -------------------------------------------------------------------------------
+// A x = sum_k h_k * (w_k . x): each term is the correlation above run on the product patch, all K terms into the same
+// accumulators.  Multipliers (MB, MC, K, H, W) and filters (FB, FC, K, h, w) broadcast independently over (B, C).
+struct SvParams {
+  BlurParams P;              // one term's geometry, exactly as blur_corr_kernel runs it
+  int K, MB, MC;
+  int woff_i, woff_j, wmap;  // adjoint: output pixel (i, j) takes the multiplier w[map(i + woff_i)][map(j + woff_j)] (H x W plane)
+  int Hm, Wm;                // multiplier plane
+  int xs;                    // forward: 1 = the x patch is staged once in shared memory, 0 = x is re-read through L1 / L2 for every k
+};
+
+// Forward.  Per k: stage filter k (flipped) and the product patch w_k[map(e)] * x[map(e)] (the reference pads w_k . x, so a padded
+// position holds exactly that product), then the window loop.  Shared memory: ks, the product patch, and (xs) the x patch.
+__global__ void __launch_bounds__(256, 2) svblur_fwd_kernel(const __grid_constant__ tt::TileMap tmap, int use_tma,
+                                                         const float* __restrict__ x, const float* __restrict__ mult,
+                                                         const float* __restrict__ filt, float* __restrict__ y, SvParams S) {
+  const BlurParams& P = S.P;
+  DINVK_DYN_SMEM(float, smem);
+  const int PH = BL_T + P.h - 1;
+  float* ks = smem;
+  float* prod = align128(smem + P.h * P.wp);
+  float* xp = align128(prod + PH * P.PW);
+  const int tid = threadIdx.x;
+  const int bc = blockIdx.y;
+  const int b = bc / P.C, c = bc - b * P.C;
+  const int i0 = (blockIdx.x / P.tiles_x) * BL_T, j0 = (blockIdx.x % P.tiles_x) * BL_T;
+  const long long plane = (long long)P.Hin * P.Win;
+  const float* src = x + (long long)bc * plane;
+  const float* wb = mult + ((long long)(S.MB == 1 ? 0 : b) * S.MC + (S.MC == 1 ? 0 : c)) * S.K * plane;
+  const float* fb = filt + ((long long)(P.FB == 1 ? 0 : b) * P.FC + (P.FC == 1 ? 0 : c)) * S.K * P.h * P.w;
+  if (S.xs) stage_patch(xp, &tmap, use_tma, src, P, i0, j0, bc);
+
+  const int tx = tid & 15, ty = tid >> 4;
+  float acc[4][4];
+#pragma unroll
+  for (int r = 0; r < 4; ++r)
+#pragma unroll
+    for (int q = 0; q < 4; ++q) acc[r][q] = 0.f;
+  for (int k = 0; k < S.K; ++k) {
+    __syncthreads();  // the window loop of term k - 1 is done with ks and prod (k = 0: the x patch has landed)
+    stage_filter(ks, fb + (long long)k * P.h * P.w, P);
+    const float* wk = wb + k * plane;
+    for (int idx = tid; idx < PH * P.PW; idx += 256) {
+      const int pr = idx / P.PW, pc = idx - pr * P.PW;
+      bool okr, okc;
+      const int gi = map_index(i0 + pr + P.off_i, P.Hin, P.map, okr);
+      const int gj = map_index(j0 + pc + P.off_j, P.Win, P.map, okc);
+      float v = 0.f;
+      if (okr && okc) {
+        const long long g = (long long)gi * P.Win + gj;
+        v = (S.xs ? xp[idx] : __ldg(src + g)) * __ldg(wk + g);
+      }
+      prod[idx] = v;
+    }
+    __syncthreads();
+    window_fma(prod, ks, P, tx, ty, acc);
+  }
+  store_tile(y + (long long)bc * P.Hout * P.Wout, acc, P, i0, j0, tx, ty);
+}
+
+// Adjoint.  The y patch is staged once; per k the correlation with the unflipped h_k goes into a partial block that is scaled by
+// w_k at the output pixel and added to the totals.  On the extended (H+h-1, W+w-1) domain of replicate / reflect the output pixel e
+// takes w_k[map(e)]: the fold sums the e with map(e) = p, over which w_k[p] is constant, so scaling before the fold is exact.
+__global__ void __launch_bounds__(256) svblur_adj_kernel(const __grid_constant__ tt::TileMap tmap, int use_tma,
+                                                         const float* __restrict__ yin, const float* __restrict__ mult,
+                                                         const float* __restrict__ filt, float* __restrict__ out, SvParams S) {
+  const BlurParams& P = S.P;
+  DINVK_DYN_SMEM(float, smem);
+  float* ks = smem;
+  float* patch = align128(smem + P.h * P.wp);
+  const int tid = threadIdx.x;
+  const int bc = blockIdx.y;
+  const int b = bc / P.C, c = bc - b * P.C;
+  const int i0 = (blockIdx.x / P.tiles_x) * BL_T, j0 = (blockIdx.x % P.tiles_x) * BL_T;
+  const long long mplane = (long long)S.Hm * S.Wm;
+  const float* wb = mult + ((long long)(S.MB == 1 ? 0 : b) * S.MC + (S.MC == 1 ? 0 : c)) * S.K * mplane;
+  const float* fb = filt + ((long long)(P.FB == 1 ? 0 : b) * P.FC + (P.FC == 1 ? 0 : c)) * S.K * P.h * P.w;
+  stage_patch(patch, &tmap, use_tma, yin + (long long)bc * P.Hin * P.Win, P, i0, j0, bc);
+
+  const int tx = tid & 15, ty = tid >> 4;
+  int mi[4], mj[4];  // multiplier row / column of this thread's outputs (clamped to 0 past the output edge; never stored)
+#pragma unroll
+  for (int e = 0; e < 4; ++e) {
+    bool ok;
+    mi[e] = map_index(i0 + ty * 4 + e + S.woff_i, S.Hm, S.wmap, ok);
+    mj[e] = map_index(j0 + tx * 4 + e + S.woff_j, S.Wm, S.wmap, ok);
+  }
+  float tot[4][4];
+#pragma unroll
+  for (int r = 0; r < 4; ++r)
+#pragma unroll
+    for (int q = 0; q < 4; ++q) tot[r][q] = 0.f;
+  for (int k = 0; k < S.K; ++k) {
+    __syncthreads();  // the window loop of term k - 1 is done with ks
+    stage_filter(ks, fb + (long long)k * P.h * P.w, P);
+    __syncthreads();
+    float part[4][4];
+#pragma unroll
+    for (int r = 0; r < 4; ++r)
+#pragma unroll
+      for (int q = 0; q < 4; ++q) part[r][q] = 0.f;
+    window_fma(patch, ks, P, tx, ty, part);
+    const float* wk = wb + k * mplane;
+#pragma unroll
+    for (int r = 0; r < 4; ++r)
+#pragma unroll
+      for (int q = 0; q < 4; ++q) tot[r][q] = fmaf(part[r][q], __ldg(wk + (long long)mi[r] * S.Wm + mj[q]), tot[r][q]);
+  }
+  store_tile(out + (long long)bc * P.Hout * P.Wout, tot, P, i0, j0, tx, ty);
+}
+
 // transpose of replicate / reflect padding: x[p,q] = sum over the extended indices that the padding maps onto (p,q)
 // z is the extended image (He = H + h - 1 rows starting at extended index a_min = h/2 - h + 1; same for columns)
 __device__ __forceinline__ int preimages(int p, int n, int amin, int amax, int mode, int* start, int* count) {
@@ -170,8 +377,8 @@ __global__ void __launch_bounds__(256) blur_fold_kernel(const float* __restrict_
   x[(long long)bc * H * W + idx] = acc;
 }
 
-static int run_corr(const float* in, const float* filt, float* out, int B, int C, int Hin, int Win, int Hout, int Wout,
-                    int FB, int FC, int h, int w, int flip, int off_i, int off_j, int map, void* stream) {
+static BlurParams corr_params(int C, int Hin, int Win, int Hout, int Wout, int FB, int FC, int h, int w, int flip, int off_i, int off_j,
+                              int map) {
   BlurParams P;
   // A tensor-map box has to start on a 16-byte boundary of the image row.  Tiles start at multiples of 64 columns, so the patch
   // origin j0 + off_j is aligned iff off_j is a multiple of 4: prepend shift = off_j mod 4 zero taps to the filter rows and move
@@ -183,18 +390,81 @@ static int run_corr(const float* in, const float* filt, float* out, int B, int C
   P.FB = FB; P.FC = FC; P.flip = flip; P.off_i = off_i; P.off_j = off_j; P.map = map;
   P.PW = BL_T + P.wp + 4;  // window reads reach column tx*4 + wp + 3
   P.tiles_x = ceil_div(Wout, BL_T);
-  const size_t smem = sizeof(float) * ((size_t)h * P.wp + (size_t)(BL_T + h - 1) * P.PW) + 128;
-  if (smem > 200 * 1024) return set_error(DINVK_EUNSUPPORTED, "blur: filter %dx%d too large for the tiled kernel", h, w);
+  return P;
+}
+
+constexpr size_t BL_SMEM_BUDGET = 200 * 1024;
+
+static size_t filter_bytes(const BlurParams& P) { return sizeof(float) * (size_t)P.h * P.wp; }
+static size_t patch_bytes(const BlurParams& P) { return sizeof(float) * (size_t)(BL_T + P.h - 1) * P.PW; }
+
+// grid + tensor map of one tiled launch over B*C planes of `in` (Hin x Win); use_tma = 0 when the map cannot be built
+static int tile_grid(const BlurParams& P, int B, int C, const float* in, bool want_tma, dim3* grid, tt::TileMap* tmap, int* use_tma) {
+  const long long tiles = (long long)P.tiles_x * ceil_div(P.Hout, BL_T);
+  if ((long long)B * C > 65535 || tiles > 2147483647LL) return set_error(DINVK_EINVAL, "blur: grid too large");
+  *grid = dim3((unsigned)tiles, B * C);
+  *tmap = tt::TileMap();
+  *use_tma = 0;
+#ifndef DINVK_EMUL
+  if (want_tma && !getenv("DINVK_NO_TMA_STAGING"))
+    *use_tma = tt::make_map_f32(tmap, in, P.Win, P.Hin, B * C, P.PW, BL_T + P.h - 1) ? 1 : 0;
+#else
+  (void)in; (void)want_tma;
+#endif
+  return DINVK_OK;
+}
+
+static int run_corr(const float* in, const float* filt, float* out, int B, int C, int Hin, int Win, int Hout, int Wout,
+                    int FB, int FC, int h, int w, int flip, int off_i, int off_j, int map, void* stream) {
+  const BlurParams P = corr_params(C, Hin, Win, Hout, Wout, FB, FC, h, w, flip, off_i, off_j, map);
+  const size_t smem = filter_bytes(P) + patch_bytes(P) + 128;
+  if (smem > BL_SMEM_BUDGET) return set_error(DINVK_EUNSUPPORTED, "blur: filter %dx%d too large for the tiled kernel", h, w);
   int rc = allow_smem(blur_corr_kernel, smem);
   if (rc) return rc;
-  const long long tiles = (long long)P.tiles_x * ceil_div(Hout, BL_T);
-  if ((long long)B * C > 65535 || tiles > 2147483647LL) return set_error(DINVK_EINVAL, "blur: grid too large");
-  tt::TileMap tmap = tt::TileMap();
-  int use_tma = 0;
-#ifndef DINVK_EMUL
-  if (!getenv("DINVK_NO_TMA_STAGING")) use_tma = tt::make_map_f32(&tmap, in, Win, Hin, B * C, P.PW, BL_T + h - 1) ? 1 : 0;
-#endif
-  DINVK_LAUNCH(blur_corr_kernel, dim3((unsigned)tiles, B * C), dim3(256), smem, stream, tmap, use_tma, in, filt, out, P);
+  dim3 grid;
+  tt::TileMap tmap;
+  int use_tma;
+  if ((rc = tile_grid(P, B, C, in, true, &grid, &tmap, &use_tma))) return rc;
+  DINVK_LAUNCH(blur_corr_kernel, grid, dim3(256), smem, stream, tmap, use_tma, in, filt, out, P);
+  return DINVK_POST_LAUNCH();
+}
+
+// Space-varying forward: the x patch stays in shared memory next to the product patch when both fit the budget Blur uses;
+// larger filters (up to Blur's own limit) re-read x for every k instead (L1 / L2 hits: the same tile, K times).
+static int run_svblur_fwd(const float* x, const float* mult, const float* filt, float* y, int B, int C, int H, int W, int Hout,
+                          int Wout, int MB, int MC, int FB, int FC, int K, int h, int w, int off_i, int off_j, int map, void* stream) {
+  SvParams S;
+  S.P = corr_params(C, H, W, Hout, Wout, FB, FC, h, w, 1, off_i, off_j, map);
+  S.K = K; S.MB = MB; S.MC = MC; S.woff_i = 0; S.woff_j = 0; S.wmap = 0; S.Hm = H; S.Wm = W;
+  const size_t one = filter_bytes(S.P) + patch_bytes(S.P) + 128, two = one + patch_bytes(S.P) + 128;
+  if (one > BL_SMEM_BUDGET) return set_error(DINVK_EUNSUPPORTED, "svblur: filter %dx%d too large for the tiled kernel", h, w);
+  S.xs = two <= BL_SMEM_BUDGET;
+  const size_t smem = S.xs ? two : one;
+  int rc = allow_smem(svblur_fwd_kernel, smem);
+  if (rc) return rc;
+  dim3 grid;
+  tt::TileMap tmap;
+  int use_tma;
+  if ((rc = tile_grid(S.P, B, C, x, S.xs, &grid, &tmap, &use_tma))) return rc;
+  DINVK_LAUNCH(svblur_fwd_kernel, grid, dim3(256), smem, stream, tmap, use_tma, x, mult, filt, y, S);
+  return DINVK_POST_LAUNCH();
+}
+
+static int run_svblur_adj(const float* y, const float* mult, const float* filt, float* out, int B, int C, int Hin, int Win, int Hout,
+                          int Wout, int MB, int MC, int FB, int FC, int K, int h, int w, int off_i, int off_j, int map, int H, int W,
+                          int woff_i, int woff_j, int wmap, void* stream) {
+  SvParams S;
+  S.P = corr_params(C, Hin, Win, Hout, Wout, FB, FC, h, w, 0, off_i, off_j, map);
+  S.K = K; S.MB = MB; S.MC = MC; S.woff_i = woff_i; S.woff_j = woff_j; S.wmap = wmap; S.Hm = H; S.Wm = W; S.xs = 0;
+  const size_t smem = filter_bytes(S.P) + patch_bytes(S.P) + 128;
+  if (smem > BL_SMEM_BUDGET) return set_error(DINVK_EUNSUPPORTED, "svblur: filter %dx%d too large for the tiled kernel", h, w);
+  int rc = allow_smem(svblur_adj_kernel, smem);
+  if (rc) return rc;
+  dim3 grid;
+  tt::TileMap tmap;
+  int use_tma;
+  if ((rc = tile_grid(S.P, B, C, y, true, &grid, &tmap, &use_tma))) return rc;
+  DINVK_LAUNCH(svblur_adj_kernel, grid, dim3(256), smem, stream, tmap, use_tma, y, mult, filt, out, S);
   return DINVK_POST_LAUNCH();
 }
 
@@ -247,5 +517,55 @@ extern "C" int dinvk_blur_adj(const float* y, const float* filt, float* x, int B
   if ((rc = run_corr(y, filt, z, B, C, H, W, He, We, FB, FC, h, w, 0, -(h - 1), -(w - 1), 0, stream))) return rc;
   DINVK_LAUNCH(blur_fold_kernel, dim3(ceil_div((long long)H * W, 256), B * C), dim3(256), 0, stream, (const float*)z, x, H, W, h, w,
                padding == DINVK_PAD_REPLICATE ? 2 : 3);
+  return DINVK_POST_LAUNCH();
+}
+
+// ---- space-varying blur: deepinv/physics/functional/product_convolution.py:10-68 (product_convolution2d and its adjoint, the
+// bodies of SpaceVaryingBlur.A / A_adjoint, deepinv/physics/blur.py:803-849) -------------------------------------------------
+static int check_svblur_args(const void* a, const void* m, const void* f, const void* o, int B, int C, int H, int W, int MB, int MC,
+                             int FB, int FC, int K, int h, int w, int padding) {
+  DINVK_CHECK_ARG(m, "svblur: null multipliers");
+  DINVK_CHECK_ARG(K >= 1, "svblur: K = %d terms", K);
+  DINVK_CHECK_ARG((MB == 1 || MB == B) && (MC == 1 || MC == C), "svblur: multiplier batch/channel (%d,%d) must be 1 or match (%d,%d)",
+                  MB, MC, B, C);
+  return check_blur_args(a, f, o, B, C, H, W, FB, FC, h, w, padding);
+}
+
+extern "C" int dinvk_svblur_fwd(const float* x, const float* mult, const float* filt, float* y, int B, int C, int H, int W, int MB,
+                                int MC, int FB, int FC, int K, int h, int w, int padding, void* stream) {
+  int rc = check_svblur_args(x, mult, filt, y, B, C, H, W, MB, MC, FB, FC, K, h, w, padding);
+  if (rc) return rc;
+  if (B == 0) return DINVK_OK;
+  if (padding == DINVK_PAD_VALID)
+    return run_svblur_fwd(x, mult, filt, y, B, C, H, W, H - h + 1, W - w + 1, MB, MC, FB, FC, K, h, w, 0, 0, 0, stream);
+  const int map = padding == DINVK_PAD_CIRCULAR ? 1 : padding == DINVK_PAD_REPLICATE ? 2 : padding == DINVK_PAD_REFLECT ? 3 : 0;
+  return run_svblur_fwd(x, mult, filt, y, B, C, H, W, H, W, MB, MC, FB, FC, K, h, w, h / 2 - (h - 1), w / 2 - (w - 1), map, stream);
+}
+
+extern "C" size_t dinvk_svblur_adj_workspace_bytes(int B, int C, int H, int W, int h, int w, int padding) {
+  return dinvk_blur_adj_workspace_bytes(B, C, H, W, h, w, padding);
+}
+
+extern "C" int dinvk_svblur_adj(const float* y, const float* mult, const float* filt, float* x, int B, int C, int H, int W, int MB,
+                                int MC, int FB, int FC, int K, int h, int w, int padding, void* workspace, size_t workspace_bytes,
+                                void* stream) {
+  int rc = check_svblur_args(y, mult, filt, x, B, C, H, W, MB, MC, FB, FC, K, h, w, padding);
+  if (rc) return rc;
+  if (B == 0) return DINVK_OK;
+  if (padding == DINVK_PAD_VALID)
+    return run_svblur_adj(y, mult, filt, x, B, C, H - h + 1, W - w + 1, H, W, MB, MC, FB, FC, K, h, w, -(h - 1), -(w - 1), 0, H, W,
+                          0, 0, 0, stream);
+  if (padding == DINVK_PAD_CIRCULAR || padding == DINVK_PAD_CONSTANT)
+    return run_svblur_adj(y, mult, filt, x, B, C, H, W, H, W, MB, MC, FB, FC, K, h, w, -(h / 2), -(w / 2),
+                          padding == DINVK_PAD_CIRCULAR ? 1 : 0, H, W, 0, 0, 0, stream);
+  // replicate / reflect: the multiplied sum on the zero-extended domain, then ONE fold (blur_fold_kernel, as dinvk_blur_adj)
+  const size_t need = dinvk_svblur_adj_workspace_bytes(B, C, H, W, h, w, padding);
+  if (!workspace || workspace_bytes < need) return set_error(DINVK_EWORKSPACE, "dinvk_svblur_adj: workspace %zu < %zu", workspace_bytes, need);
+  float* z = reinterpret_cast<float*>(((uintptr_t)workspace + 127) & ~(uintptr_t)127);
+  const int He = H + h - 1, We = W + w - 1, mode = padding == DINVK_PAD_REPLICATE ? 2 : 3;
+  if ((rc = run_svblur_adj(y, mult, filt, z, B, C, H, W, He, We, MB, MC, FB, FC, K, h, w, -(h - 1), -(w - 1), 0, H, W,
+                           h / 2 - h + 1, w / 2 - w + 1, mode, stream)))
+    return rc;
+  DINVK_LAUNCH(blur_fold_kernel, dim3(ceil_div((long long)H * W, 256), B * C), dim3(256), 0, stream, (const float*)z, x, H, W, h, w, mode);
   return DINVK_POST_LAUNCH();
 }

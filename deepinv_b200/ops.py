@@ -417,6 +417,46 @@ def blur_adj(y, filt, padding: int, H: int, W: int) -> torch.Tensor:
     return x
 
 
+def _svblur_shapes(mult, filt, B: int, C: int, H: int, W: int):
+    MB, MC, K, Hm, Wm = mult.shape
+    FB, FC, Kf, h, w = filt.shape
+    if Kf != K or (Hm, Wm) != (H, W):
+        raise ValueError(f"svblur: multipliers {tuple(mult.shape)} / filters {tuple(filt.shape)} do not match K terms on a "
+                         f"({B}, {C}, {H}, {W}) image")
+    return MB, MC, FB, FC, K, h, w
+
+
+def svblur_fwd(x, mult, filt, padding: int) -> torch.Tensor:
+    """y = sum_k filt[:, :, k] * (mult[:, :, k] . x): x (B,C,H,W), mult (MB,MC,K,H,W), filt (FB,FC,K,h,w)"""
+    dev = _require_cuda(x, mult, filt)
+    x, mult, filt = _f32c(x), _f32c(mult), _f32c(filt)
+    B, C, H, W = x.shape
+    MB, MC, FB, FC, K, h, w = _svblur_shapes(mult, filt, B, C, H, W)
+    shape = (B, C, H - h + 1, W - w + 1) if padding == _ffi.PAD_VALID else (B, C, H, W)
+    y = torch.empty(shape, dtype=torch.float32, device=dev)
+    if y.numel() == 0:
+        return y
+    check(get_lib().dinvk_svblur_fwd(_p(x), _p(mult), _p(filt), _p(y), B, C, H, W, MB, MC, FB, FC, K, h, w, padding, _stream(dev)))
+    return y
+
+
+def svblur_adj(y, mult, filt, padding: int, H: int, W: int) -> torch.Tensor:
+    """the transpose of svblur_fwd onto a (B,C,H,W) image"""
+    dev = _require_cuda(y, mult, filt)
+    y, mult, filt = _f32c(y), _f32c(mult), _f32c(filt)
+    B, C = y.shape[:2]
+    MB, MC, FB, FC, K, h, w = _svblur_shapes(mult, filt, B, C, H, W)
+    x = torch.empty(B, C, H, W, dtype=torch.float32, device=dev)
+    if x.numel() == 0:
+        return x
+    lib = get_lib()
+    nb = lib.dinvk_svblur_adj_workspace_bytes(B, C, H, W, h, w, padding)
+    ws = workspace(dev, nb, "svblur")
+    check(lib.dinvk_svblur_adj(_p(y), _p(mult), _p(filt), _p(x), B, C, H, W, MB, MC, FB, FC, K, h, w, padding, _p(ws), ws.numel(),
+                               _stream(dev)))
+    return x
+
+
 # --------------------------------------------------------------------------------------------
 # denoiser convolutions, bf16 tensor-core path (NHWC bf16 activations)
 # --------------------------------------------------------------------------------------------

@@ -7,6 +7,8 @@ convolution.py:761-787); `use_fft=True` routes the circular case through the spe
 and its rfft2-domain U/V methods, but A / A_adjoint / A_adjoint_A / prox_l2 / A_dagger are single
 fused launches of `dinvk_spectral` on PAIRS of real images packed as one complex image (a real
 filter commutes with the packing), so a (B,C,H,W) batch costs B*C/2 complex 2-D transforms.
+`SpaceVaryingBlur` (blur.py:740-868) is the product convolution sum_k h_k * (w_k . x) on one fused kernel per direction
+(`dinvk_svblur_fwd / _adj`, csrc/blur.cu).
 """
 from __future__ import annotations
 
@@ -77,6 +79,45 @@ class Blur(LinearPhysics):
             self.register_buffer("filter", filter)
             filter = None
         super().update_parameters(filter=filter, **kwargs)
+
+
+class SpaceVaryingBlur(LinearPhysics):
+    r"""y = sum_k h_k * (w_k . x), space-varying blur by product convolution (blur.py:740-868).
+
+    :param torch.Tensor filters: h_k, (b, c, K, h, w) with b in {1, B}, c in {1, C}, h <= H and w <= W.
+    :param torch.Tensor multipliers: w_k, (b, c, K, H, W), broadcast over (B, C) independently of the filters.
+    :param str padding: 'valid', 'circular', 'replicate', 'reflect' or 'constant'.
+    :param bool use_fft: stored as in the reference, where it selects FFT convolutions: the same operator up to rounding.
+        Both values run the direct fused kernel here.
+
+    `A` and `A_adjoint` take ``filters=``, ``multipliers=`` and ``padding=`` and store them; gradients flow to x only.
+    `A_dagger`, `prox_l2` and the norm estimate are the CG / power-method versions of LinearPhysics."""
+
+    def __init__(self, filters: Tensor = None, multipliers: Tensor = None, padding: str = "valid", use_fft: bool = False,
+                 device="cpu", **kwargs):
+        super().__init__(device=device, **kwargs)
+        self.register_buffer("filters", filters)
+        self.register_buffer("multipliers", multipliers)
+        self.padding = padding
+        self.use_fft = use_fft
+        self.to(device)
+
+    def A(self, x: Tensor, filters: Tensor = None, multipliers: Tensor = None, padding: str = None, **kwargs) -> Tensor:
+        from . import functional as dF
+
+        self.update_parameters(filters, multipliers, padding, **kwargs)
+        return dF.product_convolution2d(x, self.multipliers, self.filters, self.padding, use_fft=self.use_fft)
+
+    def A_adjoint(self, y: Tensor, filters: Tensor = None, multipliers: Tensor = None, padding: str = None, **kwargs) -> Tensor:
+        from . import functional as dF
+
+        self.update_parameters(filters=filters, multipliers=multipliers, padding=padding, **kwargs)
+        return dF.product_convolution2d_adjoint(y, self.multipliers, self.filters, self.padding, use_fft=self.use_fft)
+
+    def update_parameters(self, filters: Tensor = None, multipliers: Tensor = None, padding: str = None, **kwargs):
+        if padding is not None:
+            self.padding = padding
+        super().update_parameters(filters=filters, multipliers=multipliers, **kwargs)
 
 
 class BlurFFT(DecomposablePhysics):

@@ -1,7 +1,8 @@
-"""Filter constructors used by Blur / BlurFFT / Downsampling (deepinv/physics/functional/blur.py:137-372,552-583).
+"""Filter constructors used by Blur / BlurFFT / Downsampling (deepinv/physics/functional/blur.py:137-372,552-583), and the
+product convolution of SpaceVaryingBlur (deepinv/physics/functional/product_convolution.py:10-68).
 
-Host-side parameter generation (a few hundred taps): plain torch on whatever device is asked for; the operators that
-consume these filters run on the libdinvk kernels."""
+Filter generation is host-side (a few hundred taps): plain torch on whatever device is asked for; the operators that
+consume these filters, and the product convolution itself, run on the libdinvk kernels."""
 from __future__ import annotations
 
 from math import pi, sqrt
@@ -91,3 +92,52 @@ def bicubic_filter(factor: int = 2, device="cpu") -> torch.Tensor:
     w = w + (a * x.pow(3) - 5 * a * x.pow(2) + 8 * a * x - 4 * a) * (x > 1) * (x < 2)
     w = torch.outer(w, w)
     return (w / w.sum())[None, None]
+
+
+def _product_convolution_args(t: torch.Tensor, w: torch.Tensor, h: torch.Tensor, padding: str, H: int, W: int):
+    """the reference's failure modes, then the filters cut to the K terms the multipliers define"""
+    from .blur import _check_filter, _padding_code
+
+    code = _padding_code(padding)
+    if t.dim() != 4:
+        raise ValueError(f"Expected Tensor dimension to be 4 (2-D blur), is {t.dim()}")
+    K = w.size(2)
+    if h.size(2) < K:  # the reference indexes h[:, :, k] for every k < K
+        raise IndexError(f"index {h.size(2)} is out of bounds for dimension 2 with size {h.size(2)}")
+    h = h[:, :, :K]
+    B, C = t.shape[:2]
+    _check_filter(h, B, C)
+    # the reference multiplies x (B, C, H, W) by w[:, :, k]: a shape that does not broadcast raises torch's RuntimeError
+    if torch.broadcast_shapes((B, C, H, W), w[:, :, 0].shape) != (B, C, H, W):
+        raise RuntimeError(f"multipliers of shape {tuple(w.shape)} do not broadcast to images of shape {(B, C, H, W)}")
+    if tuple(w.shape[-2:]) != (H, W):
+        w = w.expand(*w.shape[:3], H, W)
+    return w, h, code
+
+
+def product_convolution2d(x: torch.Tensor, w: torch.Tensor, h: torch.Tensor, padding: str = "valid",
+                          use_fft: bool = False) -> torch.Tensor:
+    r"""y = sum_k h_k * (w_k . x) (product_convolution.py:10-41): x (B, C, H, W), multipliers w (b, c, K, H, W), filters
+    h (b', c', K, h, w), b, b' in {1, B} and c, c' in {1, C}.  One fused kernel (`dinvk_svblur_fwd`) for every padding;
+    `use_fft` selects the reference's FFT convolutions, the same operator up to rounding, and runs the same kernel here."""
+    from .. import ops
+    from .forward import linear_apply
+
+    H, W = x.shape[-2:]
+    w, h, code = _product_convolution_args(x, w, h, padding, H, W)
+    return linear_apply(x, lambda t: ops.svblur_fwd(t, w, h, code), lambda t: ops.svblur_adj(t, w, h, code, H, W))
+
+
+def product_convolution2d_adjoint(y: torch.Tensor, w: torch.Tensor, h: torch.Tensor, padding: str = "valid",
+                                  use_fft: bool = False) -> torch.Tensor:
+    r"""x = sum_k w_k . (h_k^T * y) (product_convolution.py:44-68), one fused kernel (`dinvk_svblur_adj`).  The image size
+    follows from y and h as in the reference: (H + h - 1, W + w - 1) for valid padding, y's own size otherwise."""
+    from .. import ops
+    from .forward import linear_apply
+
+    if y.dim() != 4:
+        raise ValueError(f"Expected Tensor dimension to be 4 (2-D blur), is {y.dim()}")
+    fh, fw = h.shape[-2:]
+    H, W = (y.shape[-2] + fh - 1, y.shape[-1] + fw - 1) if padding.lower() == "valid" else tuple(y.shape[-2:])
+    w, h, code = _product_convolution_args(y, w, h, padding, H, W)
+    return linear_apply(y, lambda t: ops.svblur_adj(t, w, h, code, H, W), lambda t: ops.svblur_fwd(t, w, h, code))

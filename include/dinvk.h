@@ -218,6 +218,18 @@ int dinvk_blur_adj(const float* y, const float* filt, float* x, int B, int C, in
                    int FB, int FC, int h, int w, int padding,
                    void* workspace, size_t workspace_bytes, void* stream);
 
+/* Space-varying blur, the product convolution y = sum_{k<K} h_k * (w_k . x) and its adjoint
+ * x = sum_k w_k . (h_k^T * y) (deepinv/physics/functional/product_convolution.py:10-68).
+ * x (B,C,H,W), multipliers (MB,MC,K,H,W), filters (FB,FC,K,h,w); MB, FB in {1,B} and MC, FC in {1,C}
+ * independently.  Shapes and paddings otherwise as dinvk_blur_fwd / dinvk_blur_adj; the adjoint needs
+ * the same workspace as dinvk_blur_adj.  One launch (two for the replicate / reflect adjoint), no atomics. */
+int dinvk_svblur_fwd(const float* x, const float* mult, const float* filt, float* y, int B, int C, int H, int W,
+                     int MB, int MC, int FB, int FC, int K, int h, int w, int padding, void* stream);
+size_t dinvk_svblur_adj_workspace_bytes(int B, int C, int H, int W, int h, int w, int padding);
+int dinvk_svblur_adj(const float* y, const float* mult, const float* filt, float* x, int B, int C, int H, int W,
+                     int MB, int MC, int FB, int FC, int K, int h, int w, int padding,
+                     void* workspace, size_t workspace_bytes, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Denoiser convolutions (deepinv/models/drunet.py:200-210,323-433; dncnn.py:116-131)
  * ------------------------------------------------------------------------------------------
