@@ -80,6 +80,10 @@ _SIGNATURES = {
     "dinvk_tv_stencil": (c_int, [c_int, c_void_p, c_void_p] + [c_int] * 4 + [c_void_p]),
     "dinvk_tv_fn": (c_int, [c_void_p, c_void_p] + [c_int] * 5 + [c_void_p, c_size_t, c_void_p]),
     "dinvk_tv_fn_workspace_bytes": (c_size_t, [c_int] * 4),
+    "dinvk_tgv_prox": (c_int, [c_void_p] * 9 + [c_int] * 5 + [c_float, C.c_double, C.c_double, c_int, c_int,
+                                                               c_void_p, c_size_t, c_void_p]),
+    "dinvk_tgv_prox_workspace_bytes": (c_size_t, [c_int] * 4),
+    "dinvk_tgv_block": (c_int, [C.POINTER(c_int), C.POINTER(c_int)]),
 }
 
 

@@ -13,6 +13,10 @@
 // valid and only it is written back.  Every pixel is the same formula on the same inputs whatever T and K are, so the
 // choice of T and K changes no output bit.
 //
+// tgv_cp_kernel does the same for the second-order TGV prox (TGVDenoiser.forward, deepinv/models/tgv.py:93-213, 2-D;
+// epsilon / epsilon_adjoint tgv.py:229-312), whose iteration is two stencils deep: its own T x T tile, K iterations per
+// launch and a (T + 4K)^2 region (see tgv_cp_kernel).
+//
 // Every arithmetic step is rounded separately (__fmul_rn / __fadd_rn: no FMA contraction) in the reference's order, so
 // the iterate follows the fp32 torch loop operation by operation.
 #include "common.cuh"
@@ -22,6 +26,12 @@
 #endif
 #ifndef DINVK_TV_BLOCK
 #define DINVK_TV_BLOCK 4
+#endif
+#ifndef DINVK_TGV_TILE
+#define DINVK_TGV_TILE 56
+#endif
+#ifndef DINVK_TGV_BLOCK
+#define DINVK_TGV_BLOCK 2
 #endif
 
 #ifdef DINVK_EMUL
@@ -40,7 +50,6 @@ constexpr int K = DINVK_TV_BLOCK;  // iterations per launch (= halo width)
 constexpr int R = T + 2 * K;       // staged region edge
 constexpr int NT = 512;
 constexpr int PPT = (R * R + NT - 1) / NT;  // region pixels per thread
-constexpr int NW = NT / 32;
 constexpr size_t SMEM = sizeof(float) * 3 * R * R;  // v (R^2) + u2 (2 R^2)
 static_assert(R % 2 == 0, "u2 rows must stay 8-byte aligned");
 
@@ -88,9 +97,90 @@ __device__ __forceinline__ double warp_sum(double v) {
   return v;
 }
 
-__global__ void __launch_bounds__(NT) tv_cp_kernel(Params p) {
-  __shared__ double red[NW][2 * K];
+// The end of a launch of tv_cp_kernel or tgv_cp_kernel (KB iterations per launch, NTB threads): this CTA's share of the
+// break test goes to its own slot (no float atomics: the sums are reproducible run to run), and the last CTA to finish
+// (atomic ticket) adds the slots in CTA order in fp64, applies the reference's test and writes the control block.
+// accd[s] sums (x_prev - x2)^2 and accn[s] the denominator's squares over the CTA's core after sub-iteration s.
+// EPS_OUTSIDE selects the denominator: TGV's ||x2|| + 1e-12 (tgv.py:162-164) rather than TV's ||x2 + 1e-12||, whose
+// 1e-12 the caller has already added inside accn (tv.py:139-141).
+template <int KB, int NTB, bool EPS_OUTSIDE>
+__device__ __forceinline__ void finish_launch(const double (&accd)[KB], const double (&accn)[KB], Ctrl* ctrl, double* slots,
+                                              int n_cta, int n_it_max, float crit, int it0, int n, int out, bool replay) {
+  constexpr int NWB = NTB / 32;
+  __shared__ double red[NWB][2 * KB];
+  __shared__ double tot[2 * KB];
   __shared__ int s_last;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+#pragma unroll
+  for (int s = 0; s < KB; ++s) {
+    const double d = warp_sum(accd[s]), e = warp_sum(accn[s]);
+    if (lane == 0) {
+      red[warp][s] = d;
+      red[warp][KB + s] = e;
+    }
+  }
+  __syncthreads();
+  if (tid < 2 * KB) {
+    double v = 0.0;
+    for (int w = 0; w < NWB; ++w) v += red[w][tid];
+    slots[(long long)blockIdx.x * 2 * KB + tid] = v;
+  }
+  tv_fence();
+  __syncthreads();
+  if (tid == 0) s_last = atomicAdd(&ctrl->ticket, 1) == n_cta - 1;
+  __syncthreads();
+  if (!s_last) return;
+
+  // last CTA: whole-tensor norms per sub-iteration, summed over the slots in CTA order in fp64
+  tv_fence();
+  for (int j = 0; j < 2 * KB; ++j) {
+    double v = 0.0;
+    for (int c = tid; c < n_cta; c += NTB) v += tv_ldcg(slots + (long long)c * 2 * KB + j);
+    v = warp_sum(v);
+    if (lane == 0) red[warp][0] = v;
+    __syncthreads();
+    if (tid == 0) {
+      double t = 0.0;
+      for (int w = 0; w < NWB; ++w) t += red[w][0];
+      tot[j] = t;
+    }
+    __syncthreads();
+  }
+  if (tid == 0) {
+    if (replay) {
+      ctrl->it_done = it0 + n;
+      ctrl->cur = out;
+      ctrl->status = FINISHED;
+    } else {
+      // the reference breaks after iteration it (0-based, counted in every call) when it > 1 and rel_err < crit, in fp32
+      int j = -1;
+      for (int s = 0; s < n; ++s) {
+        if (it0 + s < 2) continue;
+        const float num = (float)sqrt(tot[s]), den = (float)sqrt(tot[KB + s]);
+        const float rel = num / (EPS_OUTSIDE ? __fadd_rn(den, 1e-12f) : den);
+        if (rel < crit) { j = s; break; }
+      }
+      if (j < 0) {
+        ctrl->it_done = it0 + n;
+        ctrl->cur = out;
+        ctrl->status = it0 + n >= n_it_max ? FINISHED : RUNNING;
+      } else if (j == n - 1) {
+        ctrl->it_done = it0 + n;
+        ctrl->cur = out;
+        ctrl->conv_j1 = j + 1;
+        ctrl->status = FINISHED;
+      } else {
+        // converged inside the block: the next launch recomputes j + 1 iterations from this launch's (intact) input
+        ctrl->replay_n = j + 1;
+        ctrl->conv_j1 = j + 1;
+        ctrl->status = REPLAY;
+      }
+    }
+    ctrl->ticket = 0;
+  }
+}
+
+__global__ void __launch_bounds__(NT) tv_cp_kernel(Params p) {
   // Every CTA reads the control block before any CTA of this launch can change it: only the last CTA to finish writes it.
   Ctrl* ctrl = p.ctrl;
   const int status = ctrl->status;
@@ -207,78 +297,255 @@ __global__ void __launch_bounds__(NT) tv_cp_kernel(Params p) {
       uout[g] = U[idx];
     }
   }
+  // ||x_prev - x2|| / ||x2 + 1e-12|| < crit (tv.py:139-145)
+  finish_launch<K, NT, false>(accd, accn, ctrl, p.slots, p.n_cta, p.n_it_max, p.crit, it0, n, out, replay);
+}
 
-  // this CTA's share of the break test, one slot per CTA (no float atomics: the sums are reproducible run to run)
-  const int lane = tid & 31, warp = tid >> 5;
+}  // namespace tv
+
+// ---- TGV prox ------------------------------------------------------------------------------------------------------
+
+namespace tgv {
+using tv::Ctrl;
+using tv::FINISHED;
+using tv::REPLAY;
+
+constexpr int T = DINVK_TGV_TILE;   // owned tile edge
+constexpr int K = DINVK_TGV_BLOCK;  // iterations per launch (the halo is 2K wide)
+constexpr int R = T + 4 * K;        // staged region edge
+constexpr int NT = 512;
+constexpr int PPT = (R * R + NT - 1) / NT;  // region pixels per thread
+constexpr size_t SMEM = sizeof(float) * 7 * R * R;  // u2 (4 R^2) + tmp / d (2 R^2) + v (R^2)
+static_assert(T >= 1 && K >= 1, "bad TGV tile");
+
+struct Params {
+  const float* y;
+  float* x2[2];
+  float2* r2[2];
+  float4* u2[2];
+  const float* tl1;  // (B,) tau * lambda1
+  const float* l2;   // (B,) lambda2
+  Ctrl* ctrl;
+  double* slots;     // (n_cta, 2K): per-CTA sums of (x_prev - x2)^2 and x2^2 per sub-iteration
+  int C, H, W, tiles_x, tiles_per_plane, n_cta, n_it_max;
+  float crit, tau, one_plus_tau, sigma, rho;
+};
+
+// t / max(|t|_2 / l, 1) with torch.maximum's NaN propagation (fmaxf would drop a NaN)
+__device__ __forceinline__ float proj_den(float sq, float l) {
+  const float q = sqrtf(sq) / l;
+  return q != q ? q : fmaxf(q, 1.f);
+}
+
+// One iteration of tgv.py:149-160 reads, per output pixel, fields two stencils away:
+//   tmp(q) = tau epsilon_adjoint(u2)(q)           reads u2 at q, q + e_h, q + e_w
+//   x(p) = (x2 - nabla_adjoint(tmp) + tau y) / (1 + tau), r(p) = prox_tau_fr(r2 + tmp)   read tmp at p, p - e_h, p - e_w
+//   d(q) = nabla(2x - x2)(q) - (2r - r2)(q)       reads v = 2x - x2 at q, q + e_h, q + e_w
+//   u(p) = prox_sigma_g_conj(u2 + sigma epsilon(d))(p)   reads d at p, p - e_h, p - e_w
+// so u2 stays valid on [2s, R - 2s) of the region after s iterations: with R = T + 4K the T x T core is valid after K.
+// x2 and r2 stay valid one pixel wider, which never binds.  Per region pixel: y, x2, r2 and w = 2r - r2 in the owning
+// thread's registers; u2 (one float4, the reference's (B,C,H,W,4) layout), tmp (float2, reused for d once x and r are
+// done) and v in shared memory.  Four barriered passes per iteration: tmp; x, v, x2 and r, w, r2; d; u, u2.  Pixels
+// outside the image are zero-filled when staged and never read: every stencil tests the image borders, as the
+// reference's operators do (zero last row of nabla, zero first row of epsilon, the four-term adjoints).
+__global__ void __launch_bounds__(NT) tgv_cp_kernel(Params p) {
+  Ctrl* ctrl = p.ctrl;
+  const int status = ctrl->status;
+  if (status == FINISHED) return;
+  const bool replay = status == REPLAY;
+  const int it0 = ctrl->it_done;
+  const int n = replay ? ctrl->replay_n : min(K, p.n_it_max - it0);
+  const int in = ctrl->cur, out = in ^ 1;
+  if (n <= 0) return;
+
+  const int tid = threadIdx.x;
+  const int H = p.H, W = p.W;
+  const int plane = blockIdx.x / p.tiles_per_plane, tile = blockIdx.x % p.tiles_per_plane;
+  const int h0 = (tile / p.tiles_x) * T - 2 * K, w0 = (tile % p.tiles_x) * T - 2 * K;
+  const long long off = (long long)plane * H * W;
+  const float tl1 = p.tl1[plane / p.C], l2 = p.l2[plane / p.C];
+  const float tau = p.tau, opt = p.one_plus_tau, sigma = p.sigma, rho = p.rho;
+  const float* __restrict__ yg = p.y + off;
+  const float* __restrict__ xin = (in ? p.x2[1] : p.x2[0]) + off;  // no dynamic index into the parameter block
+  const float2* __restrict__ rin = (in ? p.r2[1] : p.r2[0]) + off;
+  const float4* __restrict__ uin = (in ? p.u2[1] : p.u2[0]) + off;
+
+  DINVK_DYN_SMEM(float, sm);
+  float4* U = reinterpret_cast<float4*>(sm);             // u2
+  float2* D = reinterpret_cast<float2*>(sm + 4 * R * R);  // tmp, then d
+  float* V = sm + 6 * R * R;                             // v = 2x - x2
+
+  float yv[PPT], xv[PPT], r0[PPT], r1[PPT], w0v[PPT], w1v[PPT];
+#pragma unroll
+  for (int i = 0; i < PPT; ++i) {
+    const int idx = tid + i * NT;
+    yv[i] = xv[i] = r0[i] = r1[i] = w0v[i] = w1v[i] = 0.f;
+    if (idx < R * R) {
+      const int gh = h0 + idx / R, gw = w0 + idx % R;
+      float4 u = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (gh >= 0 && gh < H && gw >= 0 && gw < W) {
+        const long long g = (long long)gh * W + gw;
+        yv[i] = yg[g];
+        xv[i] = xin[g];
+        const float2 r = rin[g];
+        r0[i] = r.x;
+        r1[i] = r.y;
+        u = uin[g];
+      }
+      U[idx] = u;
+    }
+  }
+  __syncthreads();
+
+  double accd[K], accn[K];
 #pragma unroll
   for (int s = 0; s < K; ++s) {
-    const double d = warp_sum(accd[s]), e = warp_sum(accn[s]);
-    if (lane == 0) {
-      red[warp][s] = d;
-      red[warp][K + s] = e;
+    accd[s] = 0.0;
+    accn[s] = 0.0;
+    if (s < n) {
+      // tmp = tau * epsilon_adjoint(u2) on [2s, R - 2s - 1); each component in tgv.py:286-310 order
+#pragma unroll
+      for (int i = 0; i < PPT; ++i) {
+        const int idx = tid + i * NT;
+        const int r = idx / R, c = idx % R;
+        const int gh = h0 + r, gw = w0 + c;
+        if (idx < R * R && r >= 2 * s && r < R - 2 * s - 1 && c >= 2 * s && c < R - 2 * s - 1 && gh >= 0 && gh < H && gw >= 0 &&
+            gw < W) {
+          const float4 u = U[idx];
+          float a0 = 0.f, a1 = 0.f;
+          if (gh < H - 1) {
+            const float4 d = U[idx + R];
+            a0 = __fsub_rn(a0, d.x);
+            a1 = __fsub_rn(a1, d.z);
+          }
+          if (gh > 0) {
+            a0 = __fadd_rn(a0, u.x);
+            a1 = __fadd_rn(a1, u.z);
+          }
+          if (gw < W - 1) {
+            const float4 e = U[idx + 1];
+            a0 = __fsub_rn(a0, e.y);
+            a1 = __fsub_rn(a1, e.w);
+          }
+          if (gw > 0) {
+            a0 = __fadd_rn(a0, u.y);
+            a1 = __fadd_rn(a1, u.w);
+          }
+          D[idx] = make_float2(__fmul_rn(tau, a0), __fmul_rn(tau, a1));
+        }
+      }
+      __syncthreads();
+      // x = prox_tau_fx(x2 - nabla_adjoint(tmp), y), v = 2x - x2, x2 += rho (x - x2);
+      // r = prox_tau_fr(r2 + tmp, lambda1), w = 2r - r2, r2 += rho (r - r2)   on [2s + 1, R - 2s - 1)
+#pragma unroll
+      for (int i = 0; i < PPT; ++i) {
+        const int idx = tid + i * NT;
+        const int r = idx / R, c = idx % R;
+        const int gh = h0 + r, gw = w0 + c;
+        if (idx < R * R && r > 2 * s && r < R - 2 * s - 1 && c > 2 * s && c < R - 2 * s - 1 && gh >= 0 && gh < H && gw >= 0 &&
+            gw < W) {
+          const float2 t = D[idx];
+          float a = 0.f;  // nabla_adjoint in tv.py:202-216 order
+          if (gh < H - 1) a = __fsub_rn(a, t.x);
+          if (gh > 0) a = __fadd_rn(a, D[idx - R].x);
+          if (gw < W - 1) a = __fsub_rn(a, t.y);
+          if (gw > 0) a = __fadd_rn(a, D[idx - 1].y);
+          const float xo = xv[i];
+          const float xn = __fadd_rn(__fsub_rn(xo, a), __fmul_rn(tau, yv[i])) / opt;
+          V[idx] = __fsub_rn(__fmul_rn(2.f, xn), xo);
+          const float x2n = __fadd_rn(xo, __fmul_rn(rho, __fsub_rn(xn, xo)));
+          xv[i] = x2n;
+          if (r >= 2 * K && r < 2 * K + T && c >= 2 * K && c < 2 * K + T) {
+            const float d = __fsub_rn(xo, x2n);
+            accd[s] += (double)d * (double)d;
+            accn[s] += (double)x2n * (double)x2n;
+          }
+          // r - r / max(sqrt(s0^2 + s1^2) / (tau lambda1), 1), the last-axis sum left to right (tgv.py:76-83)
+          const float s0 = __fadd_rn(r0[i], t.x), s1 = __fadd_rn(r1[i], t.y);
+          const float m = proj_den(__fadd_rn(__fmul_rn(s0, s0), __fmul_rn(s1, s1)), tl1);
+          const float q0 = __fsub_rn(s0, s0 / m), q1 = __fsub_rn(s1, s1 / m);
+          w0v[i] = __fsub_rn(__fmul_rn(2.f, q0), r0[i]);
+          w1v[i] = __fsub_rn(__fmul_rn(2.f, q1), r1[i]);
+          r0[i] = __fadd_rn(r0[i], __fmul_rn(rho, __fsub_rn(q0, r0[i])));
+          r1[i] = __fadd_rn(r1[i], __fmul_rn(rho, __fsub_rn(q1, r1[i])));
+        }
+      }
+      __syncthreads();
+      // d = nabla(v) - w on [2s + 1, R - 2s - 2) (tmp is dead: d takes its place)
+#pragma unroll
+      for (int i = 0; i < PPT; ++i) {
+        const int idx = tid + i * NT;
+        const int r = idx / R, c = idx % R;
+        const int gh = h0 + r, gw = w0 + c;
+        if (idx < R * R && r > 2 * s && r < R - 2 * s - 2 && c > 2 * s && c < R - 2 * s - 2 && gh >= 0 && gh < H && gw >= 0 &&
+            gw < W) {
+          const float v = V[idx];
+          const float g0 = gh < H - 1 ? __fsub_rn(V[idx + R], v) : 0.f;  // nabla: zero last row / last column
+          const float g1 = gw < W - 1 ? __fsub_rn(V[idx + 1], v) : 0.f;
+          D[idx] = make_float2(__fsub_rn(g0, w0v[i]), __fsub_rn(g1, w1v[i]));
+        }
+      }
+      __syncthreads();
+      // u = prox_sigma_g_conj(u2 + sigma epsilon(d), lambda2), u2 += rho (u - u2) on [2s + 2, R - 2s - 2)
+#pragma unroll
+      for (int i = 0; i < PPT; ++i) {
+        const int idx = tid + i * NT;
+        const int r = idx / R, c = idx % R;
+        const int gh = h0 + r, gw = w0 + c;
+        if (idx < R * R && r >= 2 * s + 2 && r < R - 2 * s - 2 && c >= 2 * s + 2 && c < R - 2 * s - 2 && gh >= 0 && gh < H &&
+            gw >= 0 && gw < W) {
+          const float2 d = D[idx];
+          float e0 = 0.f, e1 = 0.f, e2 = 0.f, e3 = 0.f;  // epsilon: backward differences, zero first row / column
+          if (gh > 0) {
+            const float2 dn = D[idx - R];
+            e0 = __fsub_rn(d.x, dn.x);
+            e2 = __fsub_rn(d.y, dn.y);
+          }
+          if (gw > 0) {
+            const float2 dw = D[idx - 1];
+            e1 = __fsub_rn(d.x, dw.x);
+            e3 = __fsub_rn(d.y, dw.y);
+          }
+          const float4 uo = U[idx];
+          const float t0 = __fadd_rn(uo.x, __fmul_rn(sigma, e0)), t1 = __fadd_rn(uo.y, __fmul_rn(sigma, e1));
+          const float t2 = __fadd_rn(uo.z, __fmul_rn(sigma, e2)), t3 = __fadd_rn(uo.w, __fmul_rn(sigma, e3));
+          const float sq = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(t0, t0), __fmul_rn(t1, t1)), __fmul_rn(t2, t2)), __fmul_rn(t3, t3));
+          const float m = proj_den(sq, l2);
+          U[idx] = make_float4(__fadd_rn(uo.x, __fmul_rn(rho, __fsub_rn(t0 / m, uo.x))),
+                               __fadd_rn(uo.y, __fmul_rn(rho, __fsub_rn(t1 / m, uo.y))),
+                               __fadd_rn(uo.z, __fmul_rn(rho, __fsub_rn(t2 / m, uo.z))),
+                               __fadd_rn(uo.w, __fmul_rn(rho, __fsub_rn(t3 / m, uo.w))));
+        }
+      }
+      __syncthreads();
     }
   }
-  __syncthreads();
-  if (tid < 2 * K) {
-    double v = 0.0;
-    for (int w = 0; w < NW; ++w) v += red[w][tid];
-    p.slots[(long long)blockIdx.x * 2 * K + tid] = v;
-  }
-  tv_fence();
-  __syncthreads();
-  if (tid == 0) s_last = atomicAdd(&ctrl->ticket, 1) == p.n_cta - 1;
-  __syncthreads();
-  if (!s_last) return;
 
-  // last CTA: whole-tensor norms per sub-iteration, summed over the slots in CTA order in fp64
-  tv_fence();
-  __shared__ double tot[2 * K];
-  for (int j = 0; j < 2 * K; ++j) {
-    double v = 0.0;
-    for (int c = tid; c < p.n_cta; c += NT) v += tv_ldcg(p.slots + (long long)c * 2 * K + j);
-    v = warp_sum(v);
-    if (lane == 0) red[warp][0] = v;
-    __syncthreads();
-    if (tid == 0) {
-      double t = 0.0;
-      for (int w = 0; w < NW; ++w) t += red[w][0];
-      tot[j] = t;
+  // write back the T x T core
+  float* __restrict__ xout = (out ? p.x2[1] : p.x2[0]) + off;
+  float2* __restrict__ rout = (out ? p.r2[1] : p.r2[0]) + off;
+  float4* __restrict__ uout = (out ? p.u2[1] : p.u2[0]) + off;
+#pragma unroll
+  for (int i = 0; i < PPT; ++i) {
+    const int idx = tid + i * NT;
+    const int r = idx / R, c = idx % R;
+    const int gh = h0 + r, gw = w0 + c;
+    if (idx < R * R && r >= 2 * K && r < 2 * K + T && c >= 2 * K && c < 2 * K + T && gh < H && gw < W) {
+      const long long g = (long long)gh * W + gw;
+      xout[g] = xv[i];
+      rout[g] = make_float2(r0[i], r1[i]);
+      uout[g] = U[idx];
     }
-    __syncthreads();
   }
-  if (tid == 0) {
-    if (replay) {
-      ctrl->it_done = it0 + n;
-      ctrl->cur = out;
-      ctrl->status = FINISHED;
-    } else {
-      // the reference breaks after iteration it (0-based, counted in every call) when it > 1 and
-      // ||x_prev - x2|| / ||x2 + 1e-12|| < crit, in fp32 (tv.py:139-145)
-      int j = -1;
-      for (int s = 0; s < n; ++s) {
-        if (it0 + s < 2) continue;
-        const float rel = (float)sqrt(tot[s]) / (float)sqrt(tot[K + s]);
-        if (rel < p.crit) { j = s; break; }
-      }
-      if (j < 0) {
-        ctrl->it_done = it0 + n;
-        ctrl->cur = out;
-        ctrl->status = it0 + n >= p.n_it_max ? FINISHED : RUNNING;
-      } else if (j == n - 1) {
-        ctrl->it_done = it0 + n;
-        ctrl->cur = out;
-        ctrl->conv_j1 = j + 1;
-        ctrl->status = FINISHED;
-      } else {
-        // converged inside the block: the next launch recomputes j + 1 iterations from this launch's (intact) input
-        ctrl->replay_n = j + 1;
-        ctrl->conv_j1 = j + 1;
-        ctrl->status = REPLAY;
-      }
-    }
-    ctrl->ticket = 0;
-  }
+  // ||x_prev - x2|| / (||x2|| + 1e-12) < crit (tgv.py:162-166)
+  tv::finish_launch<K, NT, true>(accd, accn, ctrl, p.slots, p.n_cta, p.n_it_max, p.crit, it0, n, out, replay);
 }
+
+static int tiles(int n) { return (n + T - 1) / T; }
+
+}  // namespace tgv
+
+namespace tv {
 
 // ---- stencils ------------------------------------------------------------------------------------------------------
 
@@ -315,6 +582,60 @@ __global__ void __launch_bounds__(256) nabla_adjoint_kernel(const float2* __rest
     const int hw = (int)(i - plane * H * W), h = hw / W, w = hw % W;
     const float2* gp = g + plane * H * W;
     x[i] = adjoint_at([&](int hh, int ww) { return gp[(long long)hh * W + ww]; }, h, w, H, W);
+  }
+}
+
+// TGVDenoiser.epsilon (tgv.py:229-270): (…,2) -> (…,4), component 2i + j = backward difference of field component i along
+// axis j (0: H, 1: W), stored at the upper index; zero on the first row / column
+__global__ void __launch_bounds__(256) epsilon_kernel(const float2* __restrict__ f, float4* __restrict__ g, int H, int W, long long n) {
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const long long plane = i / ((long long)H * W);
+    const int hw = (int)(i - plane * H * W), h = hw / W, w = hw % W;
+    const float2 v = f[i];
+    float4 e = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (h > 0) {
+      const float2 a = f[i - W];
+      e.x = __fsub_rn(v.x, a.x);
+      e.z = __fsub_rn(v.y, a.y);
+    }
+    if (w > 0) {
+      const float2 a = f[i - 1];
+      e.y = __fsub_rn(v.x, a.x);
+      e.w = __fsub_rn(v.y, a.y);
+    }
+    g[i] = e;
+  }
+}
+
+// TGVDenoiser.epsilon_adjoint (tgv.py:272-312): (…,4) -> (…,2), each component in the reference's order of updates
+__global__ void __launch_bounds__(256) epsilon_adjoint_kernel(const float4* __restrict__ g, float2* __restrict__ f, int H, int W,
+                                                              long long n) {
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const long long plane = i / ((long long)H * W);
+    const int hw = (int)(i - plane * H * W), h = hw / W, w = hw % W;
+    const float4 u = g[i];
+    float a0 = 0.f, a1 = 0.f;
+    if (h < H - 1) {
+      const float4 d = g[i + W];
+      a0 = __fsub_rn(a0, d.x);
+      a1 = __fsub_rn(a1, d.z);
+    }
+    if (h > 0) {
+      a0 = __fadd_rn(a0, u.x);
+      a1 = __fadd_rn(a1, u.z);
+    }
+    if (w < W - 1) {
+      const float4 e = g[i + 1];
+      a0 = __fsub_rn(a0, e.y);
+      a1 = __fsub_rn(a1, e.w);
+    }
+    if (w > 0) {
+      a0 = __fadd_rn(a0, u.y);
+      a1 = __fadd_rn(a1, u.w);
+    }
+    f[i] = make_float2(a0, a1);
   }
 }
 
@@ -457,7 +778,12 @@ extern "C" int dinvk_tv_prox(const float* y, float* x2_a, float* u2_a, float* x2
 
 extern "C" int dinvk_tv_stencil(int op, const float* in, float* out, int B, int C, int H, int W, void* stream) {
   DINVK_CHECK_ARG(in && out && B >= 0 && C >= 0 && H > 0 && W > 0, "dinvk_tv_stencil: bad arguments");
-  DINVK_CHECK_ARG(op >= 0 && op <= 2, "dinvk_tv_stencil: op must be 0 (nabla), 1 (nabla_adjoint) or 2 (TV subgradient)");
+  DINVK_CHECK_ARG(op >= 0 && op <= 4,
+                  "dinvk_tv_stencil: op must be 0 (nabla), 1 (nabla_adjoint), 2 (TV subgradient), 3 (epsilon) or 4 (epsilon_adjoint)");
+  if (op >= 3)
+    DINVK_CHECK_ARG((reinterpret_cast<uintptr_t>(in) & 7) == 0 && (reinterpret_cast<uintptr_t>(out) & 7) == 0 &&
+                        (reinterpret_cast<uintptr_t>(op == 3 ? out : in) & 15) == 0,
+                    "dinvk_tv_stencil: epsilon fields must be 8-byte (…,2) and 16-byte (…,4) aligned");
   const long long n = (long long)B * C * H * W;
   if (n == 0) return DINVK_OK;
   const dim3 grid(tv::stencil_grid(n));
@@ -465,9 +791,81 @@ extern "C" int dinvk_tv_stencil(int op, const float* in, float* out, int B, int 
     DINVK_LAUNCH(tv::nabla_kernel, grid, dim3(256), 0, stream, in, reinterpret_cast<float2*>(out), H, W, n);
   else if (op == 1)
     DINVK_LAUNCH(tv::nabla_adjoint_kernel, grid, dim3(256), 0, stream, reinterpret_cast<const float2*>(in), out, H, W, n);
-  else
+  else if (op == 2)
     DINVK_LAUNCH(tv::tv_grad_kernel, grid, dim3(256), 0, stream, in, out, H, W, n);
+  else if (op == 3)
+    DINVK_LAUNCH(tv::epsilon_kernel, grid, dim3(256), 0, stream, reinterpret_cast<const float2*>(in), reinterpret_cast<float4*>(out),
+                 H, W, n);
+  else
+    DINVK_LAUNCH(tv::epsilon_adjoint_kernel, grid, dim3(256), 0, stream, reinterpret_cast<const float4*>(in),
+                 reinterpret_cast<float2*>(out), H, W, n);
   return DINVK_POST_LAUNCH();
+}
+
+extern "C" int dinvk_tgv_block(int* tile, int* iters) {
+  if (tile) *tile = tgv::T;
+  if (iters) *iters = tgv::K;
+  return DINVK_OK;
+}
+
+extern "C" size_t dinvk_tgv_prox_workspace_bytes(int B, int C, int H, int W) {
+  const size_t n_cta = (size_t)std::max(B, 0) * std::max(C, 0) * tgv::tiles(std::max(H, 1)) * tgv::tiles(std::max(W, 1));
+  return tv::CTRL_BYTES + sizeof(double) * 2 * tgv::K * std::max<size_t>(n_cta, 1);
+}
+
+extern "C" int dinvk_tgv_prox(const float* y, float* x2_a, float* r2_a, float* u2_a, float* x2_b, float* r2_b, float* u2_b,
+                              const float* tl1, const float* l2, int B, int C, int H, int W, int n_it_max, float crit, double tau,
+                              double rho, int first, int n_launch, void* workspace, size_t workspace_bytes, void* stream) {
+  DINVK_CHECK_ARG(y && x2_a && r2_a && u2_a && x2_b && r2_b && u2_b && tl1 && l2 && workspace, "dinvk_tgv_prox: null pointer");
+  DINVK_CHECK_ARG(B >= 0 && C >= 0 && H > 0 && W > 0 && n_it_max >= 0 && n_launch >= 0, "dinvk_tgv_prox: bad shape");
+  DINVK_CHECK_ARG((reinterpret_cast<uintptr_t>(u2_a) & 15) == 0 && (reinterpret_cast<uintptr_t>(u2_b) & 15) == 0,
+                  "dinvk_tgv_prox: u2 buffers must be 16-byte aligned");
+  DINVK_CHECK_ARG((reinterpret_cast<uintptr_t>(r2_a) & 7) == 0 && (reinterpret_cast<uintptr_t>(r2_b) & 7) == 0 &&
+                      (reinterpret_cast<uintptr_t>(workspace) & 7) == 0,
+                  "dinvk_tgv_prox: r2 buffers and workspace must be 8-byte aligned");
+  if (workspace_bytes < dinvk_tgv_prox_workspace_bytes(B, C, H, W))
+    return set_error(DINVK_EWORKSPACE, "dinvk_tgv_prox: workspace too small");
+  const long long n_cta = (long long)B * C * tgv::tiles(H) * tgv::tiles(W);
+  DINVK_CHECK_ARG(n_cta < (1LL << 31), "dinvk_tgv_prox: too many tiles");
+  tgv::Params p;
+  p.y = y;
+  p.x2[0] = x2_a;
+  p.x2[1] = x2_b;
+  p.r2[0] = reinterpret_cast<float2*>(r2_a);
+  p.r2[1] = reinterpret_cast<float2*>(r2_b);
+  p.u2[0] = reinterpret_cast<float4*>(u2_a);
+  p.u2[1] = reinterpret_cast<float4*>(u2_b);
+  p.tl1 = tl1;
+  p.l2 = l2;
+  p.ctrl = reinterpret_cast<tv::Ctrl*>(workspace);
+  p.slots = reinterpret_cast<double*>(static_cast<char*>(workspace) + tv::CTRL_BYTES);
+  p.C = C;
+  p.H = H;
+  p.W = W;
+  p.tiles_x = tgv::tiles(W);
+  p.tiles_per_plane = tgv::tiles(H) * tgv::tiles(W);
+  p.n_cta = (int)n_cta;
+  p.n_it_max = n_it_max;
+  p.crit = crit;
+  // the reference's constants: python doubles rounded once to fp32 by torch (tgv.py:63-65, 74, 122)
+  p.tau = (float)tau;
+  p.one_plus_tau = (float)(1.0 + tau);
+  p.sigma = (float)(1.0 / tau / 72.0);  // 1 / tau / 72 in 2-D (tgv.py:121-122)
+  p.rho = (float)rho;
+  if (first) {
+    cudaError_t e = cudaMemsetAsync(workspace, 0, tv::CTRL_BYTES, (cudaStream_t)stream);
+    if (e != cudaSuccess) return set_error(DINVK_ECUDA, "dinvk_tgv_prox: memset: %s", cudaGetErrorString(e));
+  }
+  if (n_cta == 0) return DINVK_OK;
+  int rc;
+#ifndef DINVK_EMUL
+  if ((rc = raise_smem_limit(reinterpret_cast<const void*>(tgv::tgv_cp_kernel), tgv::SMEM))) return rc;
+#endif
+  for (int l = 0; l < n_launch; ++l) {
+    DINVK_LAUNCH(tgv::tgv_cp_kernel, dim3((unsigned)n_cta), dim3(tgv::NT), tgv::SMEM, stream, p);
+    if ((rc = DINVK_POST_LAUNCH())) return rc;
+  }
+  return DINVK_OK;
 }
 
 extern "C" size_t dinvk_tv_fn_workspace_bytes(int B, int C, int H, int W) {

@@ -763,3 +763,82 @@ def tv_fn(x: torch.Tensor, l1: bool = False) -> torch.Tensor:
     ws = workspace(dev, nb, "tv_fn")
     check(lib.dinvk_tv_fn(_p(out), _p(x), int(l1), B, C, H, W, _p(ws), ws.numel(), _stream(dev)))
     return out
+
+
+# --------------------------------------------------------------------------------------------
+# total generalized variation (deepinv/models/tgv.py)
+# --------------------------------------------------------------------------------------------
+def tgv_block(lib=None) -> tuple[int, int]:
+    """(T, K): the tile edge and the iterations per launch libdinvk's TGV prox was compiled with"""
+    t, k = ctypes.c_int(0), ctypes.c_int(0)
+    check((lib or get_lib()).dinvk_tgv_block(ctypes.byref(t), ctypes.byref(k)))
+    return t.value, k.value
+
+
+def tgv_prox(y: torch.Tensor, tl1: torch.Tensor, l2: torch.Tensor, x2: torch.Tensor, r2: torch.Tensor, u2: torch.Tensor,
+             tau: float = 0.01, rho: float = 1.99, n_it_max: int = 1000, crit: float = 1e-5, check_every: int = 16,
+             stats: Optional[dict] = None):
+    """TGVDenoiser iterations from the state (x2 (B,C,H,W), r2 (B,C,H,W,2), u2 (B,C,H,W,4)); tl1 = tau * lambda1 and
+    l2 = lambda2, (B,) on the device.
+
+    Returns (x2, r2, u2, iterations) with the iteration count as a 0-d int32 device tensor.  `stats`, if given, receives
+    the launch and host-synchronisation counts of this call.  Driven by `tv_drive` with the TV prox's control block.
+    """
+    dev = _require_cuda(y, tl1, l2, x2, r2, u2)
+    if y.dim() != 4:
+        raise NotImplementedError(f"the TGV prox is 2-D only: expected (B, C, H, W), got {tuple(y.shape)}")
+    y, tl1, l2 = _f32c(y), _f32c(tl1), _f32c(l2)
+    B, C, H, W = y.shape
+    if tl1.numel() != B or l2.numel() != B:
+        raise DinvkError(f"tl1 and l2 must hold one value per sample: {tl1.numel()}, {l2.numel()} values for a batch of {B}")
+    if r2.shape != (B, C, H, W, 2) or u2.shape != (B, C, H, W, 4) or x2.shape != y.shape:
+        raise DinvkError(f"TGV state shapes {tuple(x2.shape)}, {tuple(r2.shape)}, {tuple(u2.shape)} do not match y {tuple(y.shape)}")
+    # ping-pong state buffers: (a) the start state, (b) scratch; a replay needs its launch's input intact
+    xa, ra, ua = (t.float().clone(memory_format=torch.contiguous_format) for t in (x2, r2, u2))
+    xb, rb, ub = torch.empty_like(xa), torch.empty_like(ra), torch.empty_like(ua)
+    lib = get_lib()
+    nb = lib.dinvk_tgv_prox_workspace_bytes(B, C, H, W)
+    ws = torch.empty(nb, dtype=torch.uint8, device=dev)  # per call: the control block is the solve's state
+    stream = _stream(dev)
+    _, K = tgv_block(lib)
+
+    def launch(first, n):
+        check(lib.dinvk_tgv_prox(_p(y), _p(xa), _p(ra), _p(ua), _p(xb), _p(rb), _p(ub), _p(tl1), _p(l2), B, C, H, W,
+                                 int(n_it_max), float(crit), float(tau), float(rho), int(first), n, _p(ws), nb, stream))
+
+    def read_ctrl():
+        return dict(zip(TV_CTRL_FIELDS, ws[:24].view(torch.int32).tolist()))
+
+    if n_it_max <= 0 or y.numel() == 0:
+        ctrl = {"cur": 0, "launches": 0, "syncs": 0}
+        iters = torch.zeros((), dtype=torch.int32, device=dev)
+    else:
+        ctrl = tv_drive(launch, read_ctrl, n_it_max, K, check_every)
+        iters = torch.full((), ctrl["it_done"], dtype=torch.int32, device=dev)
+    if stats is not None:
+        stats.update(launches=ctrl["launches"], syncs=ctrl["syncs"], converged=bool(ctrl.get("conv_j1", 0)))
+    return (xb, rb, ub, iters) if ctrl["cur"] else (xa, ra, ua, iters)
+
+
+def tgv_epsilon(f: torch.Tensor) -> torch.Tensor:
+    """TGV's Jacobian of a vector field (B,C,H,W,2) -> (B,C,H,W,4), backward differences (tgv.py:229-270)"""
+    dev = _require_cuda(f)
+    if f.dim() != 5 or f.shape[-1] != 2:
+        raise NotImplementedError(f"epsilon is 2-D only: expected a (B, C, H, W, 2) tensor, got {tuple(f.shape)}")
+    f = _f32c(f)
+    out = torch.empty((*f.shape[:-1], 4), dtype=torch.float32, device=dev)
+    if f.numel():
+        check(get_lib().dinvk_tv_stencil(3, _p(f), _p(out), *f.shape[:-1], _stream(dev)))
+    return out
+
+
+def tgv_epsilon_adjoint(g: torch.Tensor) -> torch.Tensor:
+    """adjoint of `tgv_epsilon`, (B,C,H,W,4) -> (B,C,H,W,2) (tgv.py:272-312)"""
+    dev = _require_cuda(g)
+    if g.dim() != 5 or g.shape[-1] != 4:
+        raise NotImplementedError(f"epsilon_adjoint is 2-D only: expected a (B, C, H, W, 4) tensor, got {tuple(g.shape)}")
+    g = _f32c(g)
+    out = torch.empty((*g.shape[:-1], 2), dtype=torch.float32, device=dev)
+    if g.numel():
+        check(get_lib().dinvk_tv_stencil(4, _p(g), _p(out), *g.shape[:-1], _stream(dev)))
+    return out

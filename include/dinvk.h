@@ -349,8 +349,26 @@ size_t dinvk_tv_prox_workspace_bytes(int B, int C, int H, int W);
 int dinvk_tv_block(int* tile_host, int* iters_host);
 /* one-launch stencils: op 0 nabla (tv.py:153-181) in (B,C,H,W) -> out (B,C,H,W,2); op 1 nabla_adjoint (tv.py:183-218)
  * (B,C,H,W,2) -> (B,C,H,W); op 2 the TV subgradient nabla_adjoint(Dx / |Dx|), 0 where |Dx| = 0 (TVPrior.grad,
- * deepinv/optim/prior.py:544-572) */
+ * deepinv/optim/prior.py:544-572); op 3 TGV's epsilon (deepinv/models/tgv.py:229-270) (B,C,H,W,2) -> (B,C,H,W,4),
+ * backward differences with component 2i + j = d(field i)/d(axis j), zero first row / column; op 4 its adjoint
+ * epsilon_adjoint (tgv.py:272-312) (B,C,H,W,4) -> (B,C,H,W,2).  Ops 3 and 4 need the (…,4) field 16-byte aligned
+ * and the (…,2) field 8-byte aligned. */
 int dinvk_tv_stencil(int op, const float* in, float* out, int B, int C, int H, int W, void* stream);
+
+/* TGV prox by over-relaxed Chambolle-Pock, TGVDenoiser.forward (deepinv/models/tgv.py:93-213, 2-D).  Each launch runs
+ * up to `dinvk_tgv_block` iterations of tgv.py:149-160 on two ping-pong state buffers (x2_a, r2_a, u2_a) /
+ * (x2_b, r2_b, u2_b): x2 (B,C,H,W), r2 (B,C,H,W,2) 8-byte aligned, u2 (B,C,H,W,4) 16-byte aligned.  tl1 = tau * lambda1
+ * and l2 = lambda2 are (B,) fp32 on the device, formed by the caller as the reference forms them (tgv.py:124-143, 77).
+ * The break test is the reference's, it > 1 and ||x_prev - x2|| / (||x2|| + 1e-12) < crit over the whole tensor
+ * (tgv.py:162-170), evaluated on the device with the control block, replay and `first` / n_launch protocol of
+ * dinvk_tv_prox.  tau, rho: the reference's attributes (0.01, 1.99); sigma = 1 / tau / 72 and 1 + tau are formed in
+ * double and rounded once.  The workspace (8-byte aligned) holds the control block and the per-CTA sums. */
+int dinvk_tgv_prox(const float* y, float* x2_a, float* r2_a, float* u2_a, float* x2_b, float* r2_b, float* u2_b,
+                   const float* tl1, const float* l2, int B, int C, int H, int W, int n_it_max, float crit, double tau,
+                   double rho, int first, int n_launch, void* workspace, size_t workspace_bytes, void* stream);
+size_t dinvk_tgv_prox_workspace_bytes(int B, int C, int H, int W);
+/* the library's compile-time tile edge T and iterations per launch K of dinvk_tgv_prox (host pointers) */
+int dinvk_tgv_block(int* tile_host, int* iters_host);
 /* per-sample TV value (TVPrior.fn / TVL1Prior.fn, prior.py:507-522, 595-611): out[b] = sum |Dx| with the 2-norm over
  * the two differences (mode 0) or the 1-norm (mode 1); fp64 across the block and the chunks, deterministic */
 int dinvk_tv_fn(float* out, const float* x, int mode, int B, int C, int H, int W, void* workspace,
