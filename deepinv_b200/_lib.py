@@ -44,9 +44,10 @@ def get_lib() -> ctypes.CDLL:
     return _lib
 
 
-def check(rc: int) -> None:
+def check(rc: int, lib: ctypes.CDLL | None = None) -> None:
+    """raise the error of the library call that returned rc (of `lib`, the package's library by default)"""
     if rc != 0:
-        msg = get_lib().dinvk_last_error()
+        msg = (lib or get_lib()).dinvk_last_error()
         raise DinvkError(f"libdinvk error {rc}: {msg.decode(errors='replace') if msg else ''}")
 
 

@@ -1,24 +1,28 @@
-// tv.cu — total-variation prox (over-relaxed Chambolle-Pock, temporally blocked) and the TV stencils.
+// tv.cu — total-variation and TGV proxes (over-relaxed Chambolle-Pock, temporally blocked) and their stencils.
 //
 // Replaces
 //   TVDenoiser.forward / TVL1Denoiser         deepinv/models/tv.py:86-151, 238-239
 //   TVDenoiser.nabla / nabla_adjoint          deepinv/models/tv.py:153-218 (2-D)
+//   TGVDenoiser.forward                       deepinv/models/tgv.py:93-213 (2-D)
+//   TGVDenoiser.epsilon / epsilon_adjoint     deepinv/models/tgv.py:229-312 (2-D)
 //   TVPrior.fn / grad, TVL1Prior.fn           deepinv/optim/prior.py:507-572, 595-611
 //
-// tv_cp_kernel runs up to K Chambolle-Pock iterations per launch.  Each CTA owns a T x T tile of one (b, c) plane and
-// stages the (T + 2K)^2 region around it: y and x2 live in registers (each thread keeps the pixels it owns for the whole
-// launch), the relaxed-primal difference v = 2x - x2 and the dual u2 (one float2 per pixel, the reference's (B,C,H,W,2)
-// layout) live in shared memory.  An iteration needs u2 one pixel up / left of x and v one pixel down / right of u, so the
-// region that is still valid shrinks by one pixel per side per iteration; after K iterations exactly the T x T core is
-// valid and only it is written back.  Every pixel is the same formula on the same inputs whatever T and K are, so the
-// choice of T and K changes no output bit.
+// Both proxes run on one scaffold.  A CP kernel runs up to K iterations per launch; each CTA owns a T x T tile of one
+// (b, c) plane and stages the region HALO pixels wider on every side (Tile).  The fields each pixel only reads at itself
+// stay in the owning thread's registers for the whole launch, the fields a stencil reads at neighbours in shared memory.
+// A stencil pass is only valid on a band of the region that shrinks by one pixel per side per stencil, so each pass runs
+// over its own band (for_region) and after K iterations exactly the T x T core is valid and only it is written back.
+// Every pixel is the same formula on the same inputs whatever T and K are, so the choice of T and K changes no output bit.
+// The launch protocol is shared too: the control block at the head of the workspace says where the solve stands
+// (begin_launch), and the last CTA of a launch applies the reference's break test and writes it back (finish_launch).
 //
-// tgv_cp_kernel does the same for the second-order TGV prox (TGVDenoiser.forward, deepinv/models/tgv.py:93-213, 2-D;
-// epsilon / epsilon_adjoint tgv.py:229-312), whose iteration is two stencils deep: its own T x T tile, K iterations per
-// launch and a (T + 4K)^2 region (see tgv_cp_kernel).
+//   tv_cp_kernel    one stencil deep per iteration (nabla_adjoint, then nabla): HALO = K, region (T + 2K)^2.
+//   tgv_cp_kernel   two stencils deep (epsilon_adjoint, nabla_adjoint, nabla, epsilon): HALO = 2K, region (T + 4K)^2.
 //
-// Every arithmetic step is rounded separately (__fmul_rn / __fadd_rn: no FMA contraction) in the reference's order, so
-// the iterate follows the fp32 torch loop operation by operation.
+// The four operators are written once over an accessor (nabla, nabla_adjoint, epsilon, epsilon_adjoint); the CP kernels
+// apply them to shared memory and the standalone stencil kernels to global memory.  Every arithmetic step is rounded
+// separately (__fmul_rn / __fadd_rn: no FMA contraction) in the reference's order, so the iterate follows the fp32 torch
+// loop operation by operation.
 #include "common.cuh"
 
 #ifndef DINVK_TV_TILE
@@ -45,13 +49,85 @@ template <typename T> __device__ __forceinline__ T tv_ldcg(const T* p) { return 
 namespace dinvk {
 namespace tv {
 
-constexpr int T = DINVK_TV_TILE;   // owned tile edge
-constexpr int K = DINVK_TV_BLOCK;  // iterations per launch (= halo width)
-constexpr int R = T + 2 * K;       // staged region edge
-constexpr int NT = 512;
-constexpr int PPT = (R * R + NT - 1) / NT;  // region pixels per thread
-constexpr size_t SMEM = sizeof(float) * 3 * R * R;  // v (R^2) + u2 (2 R^2)
-static_assert(R % 2 == 0, "u2 rows must stay 8-byte aligned");
+// ---- stencils ------------------------------------------------------------------------------------------------------
+// Each operator reads its field through an accessor f(dh, dw) = the field at (h + dh, w + dw); (h, w) is the image pixel,
+// which the border tests need.
+
+// p[c + dh * row + dw]: the accessor over a field stored row by row, in shared memory (I = int) or global memory (I = long long)
+template <class P, class I>
+struct Around {
+  const P* p;
+  I c;
+  int row;
+  __device__ __forceinline__ P operator()(int dh, int dw) const { return p[c + (I)dh * row + dw]; }
+};
+template <class P, class I>
+__device__ __forceinline__ Around<P, I> around(const P* p, I c, int row) { return {p, c, row}; }
+
+// nabla (tv.py:153-181): forward differences, zero on the last row / column
+template <class X>
+__device__ __forceinline__ float2 nabla(X x, int h, int w, int H, int W) {
+  const float v = x(0, 0);
+  return make_float2(h < H - 1 ? __fsub_rn(x(1, 0), v) : 0.f, w < W - 1 ? __fsub_rn(x(0, 1), v) : 0.f);
+}
+
+// nabla_adjoint in tv.py:202-216 order: vertical component first, then horizontal; each "-= own, += previous"
+template <class G>
+__device__ __forceinline__ float nabla_adjoint(G g, int h, int w, int H, int W) {
+  float a = 0.f;
+  if (h < H - 1) a = __fsub_rn(a, g(0, 0).x);
+  if (h > 0) a = __fadd_rn(a, g(-1, 0).x);
+  if (w < W - 1) a = __fsub_rn(a, g(0, 0).y);
+  if (w > 0) a = __fadd_rn(a, g(0, -1).y);
+  return a;
+}
+
+// TGVDenoiser.epsilon (tgv.py:229-270): (…,2) -> (…,4), component 2i + j = backward difference of field component i along
+// axis j (0: H, 1: W), stored at the upper index; zero on the first row / column
+template <class F>
+__device__ __forceinline__ float4 epsilon(F f, int h, int w) {
+  const float2 v = f(0, 0);
+  float4 e = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (h > 0) {
+    const float2 a = f(-1, 0);
+    e.x = __fsub_rn(v.x, a.x);
+    e.z = __fsub_rn(v.y, a.y);
+  }
+  if (w > 0) {
+    const float2 a = f(0, -1);
+    e.y = __fsub_rn(v.x, a.x);
+    e.w = __fsub_rn(v.y, a.y);
+  }
+  return e;
+}
+
+// TGVDenoiser.epsilon_adjoint (tgv.py:272-312): (…,4) -> (…,2), each component in the reference's order of updates
+template <class G>
+__device__ __forceinline__ float2 epsilon_adjoint(G g, int h, int w, int H, int W) {
+  const float4 u = g(0, 0);
+  float a0 = 0.f, a1 = 0.f;
+  if (h < H - 1) {
+    const float4 d = g(1, 0);
+    a0 = __fsub_rn(a0, d.x);
+    a1 = __fsub_rn(a1, d.z);
+  }
+  if (h > 0) {
+    a0 = __fadd_rn(a0, u.x);
+    a1 = __fadd_rn(a1, u.z);
+  }
+  if (w < W - 1) {
+    const float4 e = g(0, 1);
+    a0 = __fsub_rn(a0, e.y);
+    a1 = __fsub_rn(a1, e.w);
+  }
+  if (w > 0) {
+    a0 = __fadd_rn(a0, u.y);
+    a1 = __fadd_rn(a1, u.w);
+  }
+  return make_float2(a0, a1);
+}
+
+// ---- the Chambolle-Pock scaffold -----------------------------------------------------------------------------------
 
 // control block at the head of the workspace; zeroed by the first launch call of a prox
 struct Ctrl {
@@ -66,15 +142,177 @@ struct Ctrl {
 enum { RUNNING = 0, FINISHED = 1, REPLAY = 2 };
 constexpr size_t CTRL_BYTES = 64;
 
-struct Params {
+// what both CP kernels take besides their state buffers and per-sample constants
+struct CpParams {
+  Ctrl* ctrl;
+  double* slots;  // (n_cta, 2K): per-CTA sums of the break test's numerator and denominator squares per sub-iteration
+  int C, H, W, tiles_x, tiles_per_plane, n_cta, n_it_max;
+  float crit, tau, one_plus_tau, sigma, rho;
+};
+
+// A CP kernel's tile: the T x T core a CTA owns, K iterations per launch, the region R x R staged around the core
+// (HALO pixels on every side) and the region pixels per thread.
+template <int T_, int K_, int HALO_>
+struct Tile {
+  static constexpr int T = T_, K = K_, HALO = HALO_, R = T + 2 * HALO, NT = 512, PPT = (R * R + NT - 1) / NT;
+  static_assert(T >= 1 && K >= 1, "bad tile");
+  static int tiles(int n) { return (n + T - 1) / T; }
+  static __device__ __forceinline__ bool core(int r, int c) { return r >= HALO && r < HALO + T && c >= HALO && c < HALO + T; }
+};
+
+// This launch's place in the solve and this CTA's place in the image
+struct Launch {
+  bool replay;
+  int it0, n, in, out;  // first iteration, iterations to run, ping-pong buffers read and written
+  int plane, h0, w0;    // (b, c) plane, image pixel of the region's top-left corner
+  long long off;        // the plane's offset in a (B, C, H, W) field
+};
+
+// Reads the control block; false: return now (the solve has finished or n_it_max is reached).  Every CTA reads the
+// control block before any CTA of this launch can change it: only the last CTA to finish writes it.
+template <class G>
+__device__ __forceinline__ bool begin_launch(const CpParams& p, Launch& l) {
+  const Ctrl* ctrl = p.ctrl;
+  const int status = ctrl->status;
+  if (status == FINISHED) return false;
+  l.replay = status == REPLAY;
+  l.it0 = ctrl->it_done;
+  l.n = l.replay ? ctrl->replay_n : min(G::K, p.n_it_max - l.it0);
+  l.in = ctrl->cur;
+  l.out = l.in ^ 1;
+  if (l.n <= 0) return false;
+  l.plane = blockIdx.x / p.tiles_per_plane;
+  const int tile = blockIdx.x % p.tiles_per_plane;
+  l.h0 = (tile / p.tiles_x) * G::T - G::HALO;
+  l.w0 = (tile % p.tiles_x) * G::T - G::HALO;
+  l.off = (long long)l.plane * p.H * p.W;
+  return true;
+}
+
+// buffer i of a ping-pong pair, at the plane's offset (no dynamic index into the parameter block)
+template <class P>
+__device__ __forceinline__ P* pick(P* const (&b)[2], int i, long long off) {
+  return (i ? b[1] : b[0]) + off;
+}
+
+// f(i, idx, r, c, gh, gw) for each of this thread's region pixels (i-th of its PPT, region index idx = r R + c, image
+// pixel (gh, gw)) whose region row and column lie in [lo, hi) and that lie inside the image.  Fully unrolled, so that
+// per-pixel arrays indexed by i stay in registers.
+template <class G, class F>
+__device__ __forceinline__ void for_region(const Launch& l, int H, int W, int lo, int hi, F&& f) {
+#pragma unroll
+  for (int i = 0; i < G::PPT; ++i) {
+    const int idx = threadIdx.x + i * G::NT;
+    const int r = idx / G::R, c = idx % G::R;
+    const int gh = l.h0 + r, gw = l.w0 + c;
+    if (idx < G::R * G::R && r >= lo && r < hi && c >= lo && c < hi && gh >= 0 && gh < H && gw >= 0 && gw < W)
+      f(i, idx, r, c, gh, gw);
+  }
+}
+
+__device__ __forceinline__ double warp_sum(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+// The end of a launch: this CTA's share of the break test goes to its own slot (no float atomics: the sums are
+// reproducible run to run), and the last CTA to finish (atomic ticket) adds the slots in CTA order in fp64, applies the
+// reference's test and writes the control block.  accd[s] sums (x_prev - x2)^2 and accn[s] the denominator's squares
+// over the CTA's core after sub-iteration s.  EPS_OUTSIDE selects the denominator: TGV's ||x2|| + 1e-12 (tgv.py:162-164)
+// rather than TV's ||x2 + 1e-12||, whose 1e-12 the caller has already added inside accn (tv.py:139-141).
+template <class G, bool EPS_OUTSIDE>
+__device__ __forceinline__ void finish_launch(const double (&accd)[G::K], const double (&accn)[G::K], const CpParams& p,
+                                              const Launch& l) {
+  constexpr int KB = G::K, NTB = G::NT, NWB = NTB / 32;
+  __shared__ double red[NWB][2 * KB];
+  __shared__ double tot[2 * KB];
+  __shared__ int s_last;
+  Ctrl* ctrl = p.ctrl;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+#pragma unroll
+  for (int s = 0; s < KB; ++s) {
+    const double d = warp_sum(accd[s]), e = warp_sum(accn[s]);
+    if (lane == 0) {
+      red[warp][s] = d;
+      red[warp][KB + s] = e;
+    }
+  }
+  __syncthreads();
+  if (tid < 2 * KB) {
+    double v = 0.0;
+    for (int w = 0; w < NWB; ++w) v += red[w][tid];
+    p.slots[(long long)blockIdx.x * 2 * KB + tid] = v;
+  }
+  tv_fence();
+  __syncthreads();
+  if (tid == 0) s_last = atomicAdd(&ctrl->ticket, 1) == p.n_cta - 1;
+  __syncthreads();
+  if (!s_last) return;
+
+  // last CTA: whole-tensor norms per sub-iteration, summed over the slots in CTA order in fp64
+  tv_fence();
+  for (int j = 0; j < 2 * KB; ++j) {
+    double v = 0.0;
+    for (int c = tid; c < p.n_cta; c += NTB) v += tv_ldcg(p.slots + (long long)c * 2 * KB + j);
+    v = warp_sum(v);
+    if (lane == 0) red[warp][0] = v;
+    __syncthreads();
+    if (tid == 0) {
+      double t = 0.0;
+      for (int w = 0; w < NWB; ++w) t += red[w][0];
+      tot[j] = t;
+    }
+    __syncthreads();
+  }
+  if (tid == 0) {
+    const int it0 = l.it0, n = l.n;
+    if (l.replay) {
+      ctrl->it_done = it0 + n;
+      ctrl->cur = l.out;
+      ctrl->status = FINISHED;
+    } else {
+      // the reference breaks after iteration it (0-based, counted in every call) when it > 1 and rel_err < crit, in fp32
+      int j = -1;
+      for (int s = 0; s < n; ++s) {
+        if (it0 + s < 2) continue;
+        const float num = (float)sqrt(tot[s]), den = (float)sqrt(tot[KB + s]);
+        const float rel = num / (EPS_OUTSIDE ? __fadd_rn(den, 1e-12f) : den);
+        if (rel < p.crit) { j = s; break; }
+      }
+      if (j < 0) {
+        ctrl->it_done = it0 + n;
+        ctrl->cur = l.out;
+        ctrl->status = it0 + n >= p.n_it_max ? FINISHED : RUNNING;
+      } else if (j == n - 1) {
+        ctrl->it_done = it0 + n;
+        ctrl->cur = l.out;
+        ctrl->conv_j1 = j + 1;
+        ctrl->status = FINISHED;
+      } else {
+        // converged inside the block: the next launch recomputes j + 1 iterations from this launch's (intact) input
+        ctrl->replay_n = j + 1;
+        ctrl->conv_j1 = j + 1;
+        ctrl->status = REPLAY;
+      }
+    }
+    ctrl->ticket = 0;
+  }
+}
+
+// ---- TV prox -------------------------------------------------------------------------------------------------------
+
+using TvTile = Tile<DINVK_TV_TILE, DINVK_TV_BLOCK, DINVK_TV_BLOCK>;
+constexpr size_t TV_SMEM = sizeof(float) * 3 * TvTile::R * TvTile::R;  // v (R^2) + u2 (2 R^2)
+static_assert(TvTile::R % 2 == 0, "u2 rows must stay 8-byte aligned");
+
+struct TvParams {
+  CpParams cp;
   const float* y;
   float* x2[2];
   float2* u2[2];
   const float* lambd;  // (B,)
-  Ctrl* ctrl;
-  double* slots;       // (n_cta, 2K): per-CTA sums of (x_prev - x2)^2 and (x2 + 1e-12)^2 per sub-iteration
-  int C, H, W, tiles_x, tiles_per_plane, n_cta, n_it_max, mode;
-  float crit, tau, one_plus_tau, sigma, rho;
+  int mode;
 };
 
 // dual projection: mode 0 isotropic u / max(|u| / lambd, 1) (tv.py:75-82), mode 1 per-component clamp (tv.py:238-239).
@@ -91,139 +329,34 @@ __device__ __forceinline__ float2 dual_proj(float2 t, float l, int mode) {
   return make_float2(ax, ay);
 }
 
-__device__ __forceinline__ double warp_sum(double v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
-// The end of a launch of tv_cp_kernel or tgv_cp_kernel (KB iterations per launch, NTB threads): this CTA's share of the
-// break test goes to its own slot (no float atomics: the sums are reproducible run to run), and the last CTA to finish
-// (atomic ticket) adds the slots in CTA order in fp64, applies the reference's test and writes the control block.
-// accd[s] sums (x_prev - x2)^2 and accn[s] the denominator's squares over the CTA's core after sub-iteration s.
-// EPS_OUTSIDE selects the denominator: TGV's ||x2|| + 1e-12 (tgv.py:162-164) rather than TV's ||x2 + 1e-12||, whose
-// 1e-12 the caller has already added inside accn (tv.py:139-141).
-template <int KB, int NTB, bool EPS_OUTSIDE>
-__device__ __forceinline__ void finish_launch(const double (&accd)[KB], const double (&accn)[KB], Ctrl* ctrl, double* slots,
-                                              int n_cta, int n_it_max, float crit, int it0, int n, int out, bool replay) {
-  constexpr int NWB = NTB / 32;
-  __shared__ double red[NWB][2 * KB];
-  __shared__ double tot[2 * KB];
-  __shared__ int s_last;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-#pragma unroll
-  for (int s = 0; s < KB; ++s) {
-    const double d = warp_sum(accd[s]), e = warp_sum(accn[s]);
-    if (lane == 0) {
-      red[warp][s] = d;
-      red[warp][KB + s] = e;
-    }
-  }
-  __syncthreads();
-  if (tid < 2 * KB) {
-    double v = 0.0;
-    for (int w = 0; w < NWB; ++w) v += red[w][tid];
-    slots[(long long)blockIdx.x * 2 * KB + tid] = v;
-  }
-  tv_fence();
-  __syncthreads();
-  if (tid == 0) s_last = atomicAdd(&ctrl->ticket, 1) == n_cta - 1;
-  __syncthreads();
-  if (!s_last) return;
-
-  // last CTA: whole-tensor norms per sub-iteration, summed over the slots in CTA order in fp64
-  tv_fence();
-  for (int j = 0; j < 2 * KB; ++j) {
-    double v = 0.0;
-    for (int c = tid; c < n_cta; c += NTB) v += tv_ldcg(slots + (long long)c * 2 * KB + j);
-    v = warp_sum(v);
-    if (lane == 0) red[warp][0] = v;
-    __syncthreads();
-    if (tid == 0) {
-      double t = 0.0;
-      for (int w = 0; w < NWB; ++w) t += red[w][0];
-      tot[j] = t;
-    }
-    __syncthreads();
-  }
-  if (tid == 0) {
-    if (replay) {
-      ctrl->it_done = it0 + n;
-      ctrl->cur = out;
-      ctrl->status = FINISHED;
-    } else {
-      // the reference breaks after iteration it (0-based, counted in every call) when it > 1 and rel_err < crit, in fp32
-      int j = -1;
-      for (int s = 0; s < n; ++s) {
-        if (it0 + s < 2) continue;
-        const float num = (float)sqrt(tot[s]), den = (float)sqrt(tot[KB + s]);
-        const float rel = num / (EPS_OUTSIDE ? __fadd_rn(den, 1e-12f) : den);
-        if (rel < crit) { j = s; break; }
-      }
-      if (j < 0) {
-        ctrl->it_done = it0 + n;
-        ctrl->cur = out;
-        ctrl->status = it0 + n >= n_it_max ? FINISHED : RUNNING;
-      } else if (j == n - 1) {
-        ctrl->it_done = it0 + n;
-        ctrl->cur = out;
-        ctrl->conv_j1 = j + 1;
-        ctrl->status = FINISHED;
-      } else {
-        // converged inside the block: the next launch recomputes j + 1 iterations from this launch's (intact) input
-        ctrl->replay_n = j + 1;
-        ctrl->conv_j1 = j + 1;
-        ctrl->status = REPLAY;
-      }
-    }
-    ctrl->ticket = 0;
-  }
-}
-
-__global__ void __launch_bounds__(NT) tv_cp_kernel(Params p) {
-  // Every CTA reads the control block before any CTA of this launch can change it: only the last CTA to finish writes it.
-  Ctrl* ctrl = p.ctrl;
-  const int status = ctrl->status;
-  if (status == FINISHED) return;
-  const bool replay = status == REPLAY;
-  const int it0 = ctrl->it_done;
-  const int n = replay ? ctrl->replay_n : min(K, p.n_it_max - it0);
-  const int in = ctrl->cur, out = in ^ 1;
-  if (n <= 0) return;
-
-  const int tid = threadIdx.x;
-  const int H = p.H, W = p.W;
-  const int plane = blockIdx.x / p.tiles_per_plane, tile = blockIdx.x % p.tiles_per_plane;
-  const int h0 = (tile / p.tiles_x) * T - K, w0 = (tile % p.tiles_x) * T - K;
-  const long long off = (long long)plane * H * W;
-  const float lam = p.lambd[plane / p.C];
-  const float tau = p.tau, opt = p.one_plus_tau, sigma = p.sigma, rho = p.rho;
-  const float* __restrict__ yg = p.y + off;
-  const float* __restrict__ xin = (in ? p.x2[1] : p.x2[0]) + off;  // no dynamic index into the parameter block
-  const float2* __restrict__ uin = (in ? p.u2[1] : p.u2[0]) + off;
+// y and x2 in the owning thread's registers; v = 2x - x2 and u2 (one float2 per pixel, the reference's (B,C,H,W,2)
+// layout) in shared memory.  An iteration needs u2 one pixel up / left of x and v one pixel down / right of u.  Pixels
+// outside the image are neither staged nor read: every stencil tests the image borders, as the reference's operators do.
+__global__ void __launch_bounds__(TvTile::NT) tv_cp_kernel(TvParams p) {
+  using G = TvTile;
+  constexpr int R = G::R, K = G::K;
+  Launch l;
+  if (!begin_launch<G>(p.cp, l)) return;
+  const int H = p.cp.H, W = p.cp.W;
+  const float lam = p.lambd[l.plane / p.cp.C];
+  const float tau = p.cp.tau, opt = p.cp.one_plus_tau, sigma = p.cp.sigma, rho = p.cp.rho;
+  const float* __restrict__ yg = p.y + l.off;
+  const float* __restrict__ xin = pick(p.x2, l.in, l.off);
+  const float2* __restrict__ uin = pick(p.u2, l.in, l.off);
 
   DINVK_DYN_SMEM(float, sm);
   float* V = sm;                                     // v = 2x - x2 of the current iteration
   float2* U = reinterpret_cast<float2*>(sm + R * R);  // u2
 
-  float yv[PPT], xv[PPT];
+  float yv[G::PPT], xv[G::PPT];
 #pragma unroll
-  for (int i = 0; i < PPT; ++i) {
-    const int idx = tid + i * NT;
-    yv[i] = 0.f;
-    xv[i] = 0.f;
-    if (idx < R * R) {
-      const int gh = h0 + idx / R, gw = w0 + idx % R;
-      float2 u = make_float2(0.f, 0.f);
-      if (gh >= 0 && gh < H && gw >= 0 && gw < W) {
-        const long long g = (long long)gh * W + gw;
-        yv[i] = yg[g];
-        xv[i] = xin[g];
-        u = uin[g];
-      }
-      U[idx] = u;
-    }
-  }
+  for (int i = 0; i < G::PPT; ++i) yv[i] = xv[i] = 0.f;
+  for_region<G>(l, H, W, 0, R, [&](int i, int idx, int, int, int gh, int gw) {
+    const long long g = (long long)gh * W + gw;
+    yv[i] = yg[g];
+    xv[i] = xin[g];
+    U[idx] = uin[g];
+  });
   __syncthreads();
 
   double accd[K], accn[K];
@@ -231,104 +364,62 @@ __global__ void __launch_bounds__(NT) tv_cp_kernel(Params p) {
   for (int s = 0; s < K; ++s) {
     accd[s] = 0.0;
     accn[s] = 0.0;
-    if (s < n) {
+    if (s < l.n) {
       // x = prox_tau_fx(x2 - tau nabla_adjoint(u2), y); v = 2x - x2; x2 += rho (x - x2)   (tv.py:131-133, 135)
-      // valid for region rows / columns [s + 1, R - s): reads u2 at [s, R - s)
-      const int lo = s + 1, hi = R - s;
-#pragma unroll
-      for (int i = 0; i < PPT; ++i) {
-        const int idx = tid + i * NT;
-        const int r = idx / R, c = idx % R;
-        const int gh = h0 + r, gw = w0 + c;
-        if (idx < R * R && r >= lo && r < hi && c >= lo && c < hi && gh >= 0 && gh < H && gw >= 0 && gw < W) {
-          // nabla_adjoint in tv.py:202-216 order: vertical component first, then horizontal; each "-= own, += previous"
-          float a = 0.f;
-          if (gh < H - 1) a = __fsub_rn(a, U[idx].x);
-          if (gh > 0) a = __fadd_rn(a, U[idx - R].x);
-          if (gw < W - 1) a = __fsub_rn(a, U[idx].y);
-          if (gw > 0) a = __fadd_rn(a, U[idx - 1].y);
-          const float xo = xv[i];
-          const float xn = __fadd_rn(__fsub_rn(xo, __fmul_rn(tau, a)), __fmul_rn(tau, yv[i])) / opt;
-          V[idx] = __fsub_rn(__fmul_rn(2.f, xn), xo);
-          const float x2n = __fadd_rn(xo, __fmul_rn(rho, __fsub_rn(xn, xo)));
-          xv[i] = x2n;
-          if (r >= K && r < K + T && c >= K && c < K + T) {
-            const float d = __fsub_rn(xo, x2n), e = __fadd_rn(x2n, 1e-12f);
-            accd[s] += (double)d * (double)d;
-            accn[s] += (double)e * (double)e;
-          }
+      // on [s + 1, R - s): reads u2 at [s, R - s)
+      for_region<G>(l, H, W, s + 1, R - s, [&](int i, int idx, int r, int c, int gh, int gw) {
+        const float a = nabla_adjoint(around(U, idx, R), gh, gw, H, W);
+        const float xo = xv[i];
+        const float xn = __fadd_rn(__fsub_rn(xo, __fmul_rn(tau, a)), __fmul_rn(tau, yv[i])) / opt;
+        V[idx] = __fsub_rn(__fmul_rn(2.f, xn), xo);
+        const float x2n = __fadd_rn(xo, __fmul_rn(rho, __fsub_rn(xn, xo)));
+        xv[i] = x2n;
+        if (G::core(r, c)) {
+          const float d = __fsub_rn(xo, x2n), e = __fadd_rn(x2n, 1e-12f);
+          accd[s] += (double)d * (double)d;
+          accn[s] += (double)e * (double)e;
         }
-      }
+      });
       __syncthreads();
       // u = prox_sigma_g_conj(u2 + sigma nabla(v), lambd); u2 += rho (u - u2)   (tv.py:134, 136)
-      // valid for [s + 1, R - s - 1): reads v at [s + 1, R - s)
-      const int hi2 = hi - 1;
-#pragma unroll
-      for (int i = 0; i < PPT; ++i) {
-        const int idx = tid + i * NT;
-        const int r = idx / R, c = idx % R;
-        const int gh = h0 + r, gw = w0 + c;
-        if (idx < R * R && r >= lo && r < hi2 && c >= lo && c < hi2 && gh >= 0 && gh < H && gw >= 0 && gw < W) {
-          const float v = V[idx];
-          const float g0 = gh < H - 1 ? __fsub_rn(V[idx + R], v) : 0.f;  // nabla: zero last row / last column
-          const float g1 = gw < W - 1 ? __fsub_rn(V[idx + 1], v) : 0.f;
-          const float2 uo = U[idx];
-          const float2 t = make_float2(__fadd_rn(uo.x, __fmul_rn(sigma, g0)), __fadd_rn(uo.y, __fmul_rn(sigma, g1)));
-          const float2 u = dual_proj(t, lam, p.mode);
-          U[idx] = make_float2(__fadd_rn(uo.x, __fmul_rn(rho, __fsub_rn(u.x, uo.x))),
-                               __fadd_rn(uo.y, __fmul_rn(rho, __fsub_rn(u.y, uo.y))));
-        }
-      }
+      // on [s + 1, R - s - 1): reads v at [s + 1, R - s)
+      for_region<G>(l, H, W, s + 1, R - s - 1, [&](int, int idx, int, int, int gh, int gw) {
+        const float2 g = nabla(around(V, idx, R), gh, gw, H, W);
+        const float2 uo = U[idx];
+        const float2 t = make_float2(__fadd_rn(uo.x, __fmul_rn(sigma, g.x)), __fadd_rn(uo.y, __fmul_rn(sigma, g.y)));
+        const float2 u = dual_proj(t, lam, p.mode);
+        U[idx] = make_float2(__fadd_rn(uo.x, __fmul_rn(rho, __fsub_rn(u.x, uo.x))),
+                             __fadd_rn(uo.y, __fmul_rn(rho, __fsub_rn(u.y, uo.y))));
+      });
       __syncthreads();
     }
   }
 
   // write back the T x T core
-  float* __restrict__ xout = (out ? p.x2[1] : p.x2[0]) + off;
-  float2* __restrict__ uout = (out ? p.u2[1] : p.u2[0]) + off;
-#pragma unroll
-  for (int i = 0; i < PPT; ++i) {
-    const int idx = tid + i * NT;
-    const int r = idx / R, c = idx % R;
-    const int gh = h0 + r, gw = w0 + c;
-    if (idx < R * R && r >= K && r < K + T && c >= K && c < K + T && gh < H && gw < W) {
-      const long long g = (long long)gh * W + gw;
-      xout[g] = xv[i];
-      uout[g] = U[idx];
-    }
-  }
+  float* __restrict__ xout = pick(p.x2, l.out, l.off);
+  float2* __restrict__ uout = pick(p.u2, l.out, l.off);
+  for_region<G>(l, H, W, G::HALO, G::HALO + G::T, [&](int i, int idx, int, int, int gh, int gw) {
+    const long long g = (long long)gh * W + gw;
+    xout[g] = xv[i];
+    uout[g] = U[idx];
+  });
   // ||x_prev - x2|| / ||x2 + 1e-12|| < crit (tv.py:139-145)
-  finish_launch<K, NT, false>(accd, accn, ctrl, p.slots, p.n_cta, p.n_it_max, p.crit, it0, n, out, replay);
+  finish_launch<G, false>(accd, accn, p.cp, l);
 }
-
-}  // namespace tv
 
 // ---- TGV prox ------------------------------------------------------------------------------------------------------
 
-namespace tgv {
-using tv::Ctrl;
-using tv::FINISHED;
-using tv::REPLAY;
+using TgvTile = Tile<DINVK_TGV_TILE, DINVK_TGV_BLOCK, 2 * DINVK_TGV_BLOCK>;
+constexpr size_t TGV_SMEM = sizeof(float) * 7 * TgvTile::R * TgvTile::R;  // u2 (4 R^2) + tmp / d (2 R^2) + v (R^2)
 
-constexpr int T = DINVK_TGV_TILE;   // owned tile edge
-constexpr int K = DINVK_TGV_BLOCK;  // iterations per launch (the halo is 2K wide)
-constexpr int R = T + 4 * K;        // staged region edge
-constexpr int NT = 512;
-constexpr int PPT = (R * R + NT - 1) / NT;  // region pixels per thread
-constexpr size_t SMEM = sizeof(float) * 7 * R * R;  // u2 (4 R^2) + tmp / d (2 R^2) + v (R^2)
-static_assert(T >= 1 && K >= 1, "bad TGV tile");
-
-struct Params {
+struct TgvParams {
+  CpParams cp;
   const float* y;
   float* x2[2];
   float2* r2[2];
   float4* u2[2];
   const float* tl1;  // (B,) tau * lambda1
   const float* l2;   // (B,) lambda2
-  Ctrl* ctrl;
-  double* slots;     // (n_cta, 2K): per-CTA sums of (x_prev - x2)^2 and x2^2 per sub-iteration
-  int C, H, W, tiles_x, tiles_per_plane, n_cta, n_it_max;
-  float crit, tau, one_plus_tau, sigma, rho;
 };
 
 // t / max(|t|_2 / l, 1) with torch.maximum's NaN propagation (fmaxf would drop a NaN)
@@ -346,55 +437,38 @@ __device__ __forceinline__ float proj_den(float sq, float l) {
 // x2 and r2 stay valid one pixel wider, which never binds.  Per region pixel: y, x2, r2 and w = 2r - r2 in the owning
 // thread's registers; u2 (one float4, the reference's (B,C,H,W,4) layout), tmp (float2, reused for d once x and r are
 // done) and v in shared memory.  Four barriered passes per iteration: tmp; x, v, x2 and r, w, r2; d; u, u2.  Pixels
-// outside the image are zero-filled when staged and never read: every stencil tests the image borders, as the
-// reference's operators do (zero last row of nabla, zero first row of epsilon, the four-term adjoints).
-__global__ void __launch_bounds__(NT) tgv_cp_kernel(Params p) {
-  Ctrl* ctrl = p.ctrl;
-  const int status = ctrl->status;
-  if (status == FINISHED) return;
-  const bool replay = status == REPLAY;
-  const int it0 = ctrl->it_done;
-  const int n = replay ? ctrl->replay_n : min(K, p.n_it_max - it0);
-  const int in = ctrl->cur, out = in ^ 1;
-  if (n <= 0) return;
-
-  const int tid = threadIdx.x;
-  const int H = p.H, W = p.W;
-  const int plane = blockIdx.x / p.tiles_per_plane, tile = blockIdx.x % p.tiles_per_plane;
-  const int h0 = (tile / p.tiles_x) * T - 2 * K, w0 = (tile % p.tiles_x) * T - 2 * K;
-  const long long off = (long long)plane * H * W;
-  const float tl1 = p.tl1[plane / p.C], l2 = p.l2[plane / p.C];
-  const float tau = p.tau, opt = p.one_plus_tau, sigma = p.sigma, rho = p.rho;
-  const float* __restrict__ yg = p.y + off;
-  const float* __restrict__ xin = (in ? p.x2[1] : p.x2[0]) + off;  // no dynamic index into the parameter block
-  const float2* __restrict__ rin = (in ? p.r2[1] : p.r2[0]) + off;
-  const float4* __restrict__ uin = (in ? p.u2[1] : p.u2[0]) + off;
+// outside the image are neither staged nor read: every stencil tests the image borders, as the reference's operators do
+// (zero last row of nabla, zero first row of epsilon, the four-term adjoints).
+__global__ void __launch_bounds__(TgvTile::NT) tgv_cp_kernel(TgvParams p) {
+  using G = TgvTile;
+  constexpr int R = G::R, K = G::K;
+  Launch l;
+  if (!begin_launch<G>(p.cp, l)) return;
+  const int H = p.cp.H, W = p.cp.W;
+  const float tl1 = p.tl1[l.plane / p.cp.C], l2 = p.l2[l.plane / p.cp.C];
+  const float tau = p.cp.tau, opt = p.cp.one_plus_tau, sigma = p.cp.sigma, rho = p.cp.rho;
+  const float* __restrict__ yg = p.y + l.off;
+  const float* __restrict__ xin = pick(p.x2, l.in, l.off);
+  const float2* __restrict__ rin = pick(p.r2, l.in, l.off);
+  const float4* __restrict__ uin = pick(p.u2, l.in, l.off);
 
   DINVK_DYN_SMEM(float, sm);
   float4* U = reinterpret_cast<float4*>(sm);             // u2
   float2* D = reinterpret_cast<float2*>(sm + 4 * R * R);  // tmp, then d
   float* V = sm + 6 * R * R;                             // v = 2x - x2
 
-  float yv[PPT], xv[PPT], r0[PPT], r1[PPT], w0v[PPT], w1v[PPT];
+  float yv[G::PPT], xv[G::PPT], r0[G::PPT], r1[G::PPT], w0v[G::PPT], w1v[G::PPT];
 #pragma unroll
-  for (int i = 0; i < PPT; ++i) {
-    const int idx = tid + i * NT;
-    yv[i] = xv[i] = r0[i] = r1[i] = w0v[i] = w1v[i] = 0.f;
-    if (idx < R * R) {
-      const int gh = h0 + idx / R, gw = w0 + idx % R;
-      float4 u = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (gh >= 0 && gh < H && gw >= 0 && gw < W) {
-        const long long g = (long long)gh * W + gw;
-        yv[i] = yg[g];
-        xv[i] = xin[g];
-        const float2 r = rin[g];
-        r0[i] = r.x;
-        r1[i] = r.y;
-        u = uin[g];
-      }
-      U[idx] = u;
-    }
-  }
+  for (int i = 0; i < G::PPT; ++i) yv[i] = xv[i] = r0[i] = r1[i] = w0v[i] = w1v[i] = 0.f;
+  for_region<G>(l, H, W, 0, R, [&](int i, int idx, int, int, int gh, int gw) {
+    const long long g = (long long)gh * W + gw;
+    yv[i] = yg[g];
+    xv[i] = xin[g];
+    const float2 r = rin[g];
+    r0[i] = r.x;
+    r1[i] = r.y;
+    U[idx] = uin[g];
+  });
   __syncthreads();
 
   double accd[K], accn[K];
@@ -402,256 +476,154 @@ __global__ void __launch_bounds__(NT) tgv_cp_kernel(Params p) {
   for (int s = 0; s < K; ++s) {
     accd[s] = 0.0;
     accn[s] = 0.0;
-    if (s < n) {
-      // tmp = tau * epsilon_adjoint(u2) on [2s, R - 2s - 1); each component in tgv.py:286-310 order
-#pragma unroll
-      for (int i = 0; i < PPT; ++i) {
-        const int idx = tid + i * NT;
-        const int r = idx / R, c = idx % R;
-        const int gh = h0 + r, gw = w0 + c;
-        if (idx < R * R && r >= 2 * s && r < R - 2 * s - 1 && c >= 2 * s && c < R - 2 * s - 1 && gh >= 0 && gh < H && gw >= 0 &&
-            gw < W) {
-          const float4 u = U[idx];
-          float a0 = 0.f, a1 = 0.f;
-          if (gh < H - 1) {
-            const float4 d = U[idx + R];
-            a0 = __fsub_rn(a0, d.x);
-            a1 = __fsub_rn(a1, d.z);
-          }
-          if (gh > 0) {
-            a0 = __fadd_rn(a0, u.x);
-            a1 = __fadd_rn(a1, u.z);
-          }
-          if (gw < W - 1) {
-            const float4 e = U[idx + 1];
-            a0 = __fsub_rn(a0, e.y);
-            a1 = __fsub_rn(a1, e.w);
-          }
-          if (gw > 0) {
-            a0 = __fadd_rn(a0, u.y);
-            a1 = __fadd_rn(a1, u.w);
-          }
-          D[idx] = make_float2(__fmul_rn(tau, a0), __fmul_rn(tau, a1));
-        }
-      }
+    if (s < l.n) {
+      // tmp = tau * epsilon_adjoint(u2) on [2s, R - 2s - 1)
+      for_region<G>(l, H, W, 2 * s, R - 2 * s - 1, [&](int, int idx, int, int, int gh, int gw) {
+        const float2 a = epsilon_adjoint(around(U, idx, R), gh, gw, H, W);
+        D[idx] = make_float2(__fmul_rn(tau, a.x), __fmul_rn(tau, a.y));
+      });
       __syncthreads();
       // x = prox_tau_fx(x2 - nabla_adjoint(tmp), y), v = 2x - x2, x2 += rho (x - x2);
       // r = prox_tau_fr(r2 + tmp, lambda1), w = 2r - r2, r2 += rho (r - r2)   on [2s + 1, R - 2s - 1)
-#pragma unroll
-      for (int i = 0; i < PPT; ++i) {
-        const int idx = tid + i * NT;
-        const int r = idx / R, c = idx % R;
-        const int gh = h0 + r, gw = w0 + c;
-        if (idx < R * R && r > 2 * s && r < R - 2 * s - 1 && c > 2 * s && c < R - 2 * s - 1 && gh >= 0 && gh < H && gw >= 0 &&
-            gw < W) {
-          const float2 t = D[idx];
-          float a = 0.f;  // nabla_adjoint in tv.py:202-216 order
-          if (gh < H - 1) a = __fsub_rn(a, t.x);
-          if (gh > 0) a = __fadd_rn(a, D[idx - R].x);
-          if (gw < W - 1) a = __fsub_rn(a, t.y);
-          if (gw > 0) a = __fadd_rn(a, D[idx - 1].y);
-          const float xo = xv[i];
-          const float xn = __fadd_rn(__fsub_rn(xo, a), __fmul_rn(tau, yv[i])) / opt;
-          V[idx] = __fsub_rn(__fmul_rn(2.f, xn), xo);
-          const float x2n = __fadd_rn(xo, __fmul_rn(rho, __fsub_rn(xn, xo)));
-          xv[i] = x2n;
-          if (r >= 2 * K && r < 2 * K + T && c >= 2 * K && c < 2 * K + T) {
-            const float d = __fsub_rn(xo, x2n);
-            accd[s] += (double)d * (double)d;
-            accn[s] += (double)x2n * (double)x2n;
-          }
-          // r - r / max(sqrt(s0^2 + s1^2) / (tau lambda1), 1), the last-axis sum left to right (tgv.py:76-83)
-          const float s0 = __fadd_rn(r0[i], t.x), s1 = __fadd_rn(r1[i], t.y);
-          const float m = proj_den(__fadd_rn(__fmul_rn(s0, s0), __fmul_rn(s1, s1)), tl1);
-          const float q0 = __fsub_rn(s0, s0 / m), q1 = __fsub_rn(s1, s1 / m);
-          w0v[i] = __fsub_rn(__fmul_rn(2.f, q0), r0[i]);
-          w1v[i] = __fsub_rn(__fmul_rn(2.f, q1), r1[i]);
-          r0[i] = __fadd_rn(r0[i], __fmul_rn(rho, __fsub_rn(q0, r0[i])));
-          r1[i] = __fadd_rn(r1[i], __fmul_rn(rho, __fsub_rn(q1, r1[i])));
+      for_region<G>(l, H, W, 2 * s + 1, R - 2 * s - 1, [&](int i, int idx, int r, int c, int gh, int gw) {
+        const float2 t = D[idx];
+        const float a = nabla_adjoint(around(D, idx, R), gh, gw, H, W);
+        const float xo = xv[i];
+        const float xn = __fadd_rn(__fsub_rn(xo, a), __fmul_rn(tau, yv[i])) / opt;
+        V[idx] = __fsub_rn(__fmul_rn(2.f, xn), xo);
+        const float x2n = __fadd_rn(xo, __fmul_rn(rho, __fsub_rn(xn, xo)));
+        xv[i] = x2n;
+        if (G::core(r, c)) {
+          const float d = __fsub_rn(xo, x2n);
+          accd[s] += (double)d * (double)d;
+          accn[s] += (double)x2n * (double)x2n;
         }
-      }
+        // r - r / max(sqrt(s0^2 + s1^2) / (tau lambda1), 1), the last-axis sum left to right (tgv.py:76-83)
+        const float s0 = __fadd_rn(r0[i], t.x), s1 = __fadd_rn(r1[i], t.y);
+        const float m = proj_den(__fadd_rn(__fmul_rn(s0, s0), __fmul_rn(s1, s1)), tl1);
+        const float q0 = __fsub_rn(s0, s0 / m), q1 = __fsub_rn(s1, s1 / m);
+        w0v[i] = __fsub_rn(__fmul_rn(2.f, q0), r0[i]);
+        w1v[i] = __fsub_rn(__fmul_rn(2.f, q1), r1[i]);
+        r0[i] = __fadd_rn(r0[i], __fmul_rn(rho, __fsub_rn(q0, r0[i])));
+        r1[i] = __fadd_rn(r1[i], __fmul_rn(rho, __fsub_rn(q1, r1[i])));
+      });
       __syncthreads();
       // d = nabla(v) - w on [2s + 1, R - 2s - 2) (tmp is dead: d takes its place)
-#pragma unroll
-      for (int i = 0; i < PPT; ++i) {
-        const int idx = tid + i * NT;
-        const int r = idx / R, c = idx % R;
-        const int gh = h0 + r, gw = w0 + c;
-        if (idx < R * R && r > 2 * s && r < R - 2 * s - 2 && c > 2 * s && c < R - 2 * s - 2 && gh >= 0 && gh < H && gw >= 0 &&
-            gw < W) {
-          const float v = V[idx];
-          const float g0 = gh < H - 1 ? __fsub_rn(V[idx + R], v) : 0.f;  // nabla: zero last row / last column
-          const float g1 = gw < W - 1 ? __fsub_rn(V[idx + 1], v) : 0.f;
-          D[idx] = make_float2(__fsub_rn(g0, w0v[i]), __fsub_rn(g1, w1v[i]));
-        }
-      }
+      for_region<G>(l, H, W, 2 * s + 1, R - 2 * s - 2, [&](int i, int idx, int, int, int gh, int gw) {
+        const float2 g = nabla(around(V, idx, R), gh, gw, H, W);
+        D[idx] = make_float2(__fsub_rn(g.x, w0v[i]), __fsub_rn(g.y, w1v[i]));
+      });
       __syncthreads();
       // u = prox_sigma_g_conj(u2 + sigma epsilon(d), lambda2), u2 += rho (u - u2) on [2s + 2, R - 2s - 2)
-#pragma unroll
-      for (int i = 0; i < PPT; ++i) {
-        const int idx = tid + i * NT;
-        const int r = idx / R, c = idx % R;
-        const int gh = h0 + r, gw = w0 + c;
-        if (idx < R * R && r >= 2 * s + 2 && r < R - 2 * s - 2 && c >= 2 * s + 2 && c < R - 2 * s - 2 && gh >= 0 && gh < H &&
-            gw >= 0 && gw < W) {
-          const float2 d = D[idx];
-          float e0 = 0.f, e1 = 0.f, e2 = 0.f, e3 = 0.f;  // epsilon: backward differences, zero first row / column
-          if (gh > 0) {
-            const float2 dn = D[idx - R];
-            e0 = __fsub_rn(d.x, dn.x);
-            e2 = __fsub_rn(d.y, dn.y);
-          }
-          if (gw > 0) {
-            const float2 dw = D[idx - 1];
-            e1 = __fsub_rn(d.x, dw.x);
-            e3 = __fsub_rn(d.y, dw.y);
-          }
-          const float4 uo = U[idx];
-          const float t0 = __fadd_rn(uo.x, __fmul_rn(sigma, e0)), t1 = __fadd_rn(uo.y, __fmul_rn(sigma, e1));
-          const float t2 = __fadd_rn(uo.z, __fmul_rn(sigma, e2)), t3 = __fadd_rn(uo.w, __fmul_rn(sigma, e3));
-          const float sq = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(t0, t0), __fmul_rn(t1, t1)), __fmul_rn(t2, t2)), __fmul_rn(t3, t3));
-          const float m = proj_den(sq, l2);
-          U[idx] = make_float4(__fadd_rn(uo.x, __fmul_rn(rho, __fsub_rn(t0 / m, uo.x))),
-                               __fadd_rn(uo.y, __fmul_rn(rho, __fsub_rn(t1 / m, uo.y))),
-                               __fadd_rn(uo.z, __fmul_rn(rho, __fsub_rn(t2 / m, uo.z))),
-                               __fadd_rn(uo.w, __fmul_rn(rho, __fsub_rn(t3 / m, uo.w))));
-        }
-      }
+      for_region<G>(l, H, W, 2 * s + 2, R - 2 * s - 2, [&](int, int idx, int, int, int gh, int gw) {
+        const float4 e = epsilon(around(D, idx, R), gh, gw);
+        const float4 uo = U[idx];
+        const float t0 = __fadd_rn(uo.x, __fmul_rn(sigma, e.x)), t1 = __fadd_rn(uo.y, __fmul_rn(sigma, e.y));
+        const float t2 = __fadd_rn(uo.z, __fmul_rn(sigma, e.z)), t3 = __fadd_rn(uo.w, __fmul_rn(sigma, e.w));
+        const float sq = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(t0, t0), __fmul_rn(t1, t1)), __fmul_rn(t2, t2)), __fmul_rn(t3, t3));
+        const float m = proj_den(sq, l2);
+        U[idx] = make_float4(__fadd_rn(uo.x, __fmul_rn(rho, __fsub_rn(t0 / m, uo.x))),
+                             __fadd_rn(uo.y, __fmul_rn(rho, __fsub_rn(t1 / m, uo.y))),
+                             __fadd_rn(uo.z, __fmul_rn(rho, __fsub_rn(t2 / m, uo.z))),
+                             __fadd_rn(uo.w, __fmul_rn(rho, __fsub_rn(t3 / m, uo.w))));
+      });
       __syncthreads();
     }
   }
 
   // write back the T x T core
-  float* __restrict__ xout = (out ? p.x2[1] : p.x2[0]) + off;
-  float2* __restrict__ rout = (out ? p.r2[1] : p.r2[0]) + off;
-  float4* __restrict__ uout = (out ? p.u2[1] : p.u2[0]) + off;
-#pragma unroll
-  for (int i = 0; i < PPT; ++i) {
-    const int idx = tid + i * NT;
-    const int r = idx / R, c = idx % R;
-    const int gh = h0 + r, gw = w0 + c;
-    if (idx < R * R && r >= 2 * K && r < 2 * K + T && c >= 2 * K && c < 2 * K + T && gh < H && gw < W) {
-      const long long g = (long long)gh * W + gw;
-      xout[g] = xv[i];
-      rout[g] = make_float2(r0[i], r1[i]);
-      uout[g] = U[idx];
-    }
-  }
+  float* __restrict__ xout = pick(p.x2, l.out, l.off);
+  float2* __restrict__ rout = pick(p.r2, l.out, l.off);
+  float4* __restrict__ uout = pick(p.u2, l.out, l.off);
+  for_region<G>(l, H, W, G::HALO, G::HALO + G::T, [&](int i, int idx, int, int, int gh, int gw) {
+    const long long g = (long long)gh * W + gw;
+    xout[g] = xv[i];
+    rout[g] = make_float2(r0[i], r1[i]);
+    uout[g] = U[idx];
+  });
   // ||x_prev - x2|| / (||x2|| + 1e-12) < crit (tgv.py:162-166)
-  tv::finish_launch<K, NT, true>(accd, accn, ctrl, p.slots, p.n_cta, p.n_it_max, p.crit, it0, n, out, replay);
+  finish_launch<G, true>(accd, accn, p.cp, l);
 }
 
-static int tiles(int n) { return (n + T - 1) / T; }
+// ---- host side of the CP proxes ------------------------------------------------------------------------------------
 
-}  // namespace tgv
-
-namespace tv {
-
-// ---- stencils ------------------------------------------------------------------------------------------------------
-
-__device__ __forceinline__ float2 nabla_at(const float* x, int h, int w, int H, int W) {
-  const float v = x[(long long)h * W + w];
-  return make_float2(h < H - 1 ? __fsub_rn(x[(long long)(h + 1) * W + w], v) : 0.f,
-                     w < W - 1 ? __fsub_rn(x[(long long)h * W + w + 1], v) : 0.f);
+template <class G>
+static size_t workspace_bytes(int B, int C, int H, int W) {
+  const size_t n_cta = (size_t)std::max(B, 0) * std::max(C, 0) * G::tiles(std::max(H, 1)) * G::tiles(std::max(W, 1));
+  return CTRL_BYTES + sizeof(double) * 2 * G::K * std::max<size_t>(n_cta, 1);
 }
 
-// nabla_adjoint in tv.py:202-216 order, g(h, w) -> component
-template <typename G>
-__device__ __forceinline__ float adjoint_at(G g, int h, int w, int H, int W) {
-  float a = 0.f;
-  if (h < H - 1) a = __fsub_rn(a, g(h, w).x);
-  if (h > 0) a = __fadd_rn(a, g(h - 1, w).x);
-  if (w < W - 1) a = __fsub_rn(a, g(h, w).y);
-  if (w > 0) a = __fadd_rn(a, g(h, w - 1).y);
-  return a;
+// What the two prox entry points share: checks the shape and the workspace, fills p.cp with the reference's constants
+// (python doubles rounded once to fp32 by torch), clears the control block on the first call of a prox and issues
+// n_launch launches of the kernel.
+template <class G, class P>
+static int run_cp(const char* name, void (*kernel)(P), size_t smem, P& p, int B, int C, int H, int W, int n_it_max, float crit,
+                  double tau, double sigma, double rho, int first, int n_launch, void* workspace, size_t workspace_bytes,
+                  void* stream) {
+  DINVK_CHECK_ARG(B >= 0 && C >= 0 && H > 0 && W > 0 && n_it_max >= 0 && n_launch >= 0, "%s: bad shape", name);
+  DINVK_CHECK_ARG((reinterpret_cast<uintptr_t>(workspace) & 7) == 0, "%s: workspace must be 8-byte aligned", name);
+  if (workspace_bytes < tv::workspace_bytes<G>(B, C, H, W)) return set_error(DINVK_EWORKSPACE, "%s: workspace too small", name);
+  const long long n_cta = (long long)B * C * G::tiles(H) * G::tiles(W);
+  DINVK_CHECK_ARG(n_cta < (1LL << 31), "%s: too many tiles", name);
+  p.cp = CpParams{reinterpret_cast<Ctrl*>(workspace), reinterpret_cast<double*>(static_cast<char*>(workspace) + CTRL_BYTES), C, H, W,
+                  G::tiles(W), G::tiles(H) * G::tiles(W), (int)n_cta, n_it_max, crit, (float)tau, (float)(1.0 + tau), (float)sigma,
+                  (float)rho};
+  if (first) {
+    cudaError_t e = cudaMemsetAsync(workspace, 0, CTRL_BYTES, (cudaStream_t)stream);
+    if (e != cudaSuccess) return set_error(DINVK_ECUDA, "%s: memset: %s", name, cudaGetErrorString(e));
+  }
+  if (n_cta == 0) return DINVK_OK;
+  int rc;
+#ifndef DINVK_EMUL
+  // opt in even at exactly 48 KB of dynamic shared memory: the static reduction buffers come on top of it
+  if ((rc = raise_smem_limit(reinterpret_cast<const void*>(kernel), smem))) return rc;
+#endif
+  for (int l = 0; l < n_launch; ++l) {
+    DINVK_LAUNCH(kernel, dim3((unsigned)n_cta), dim3(G::NT), smem, stream, p);
+    if ((rc = DINVK_POST_LAUNCH())) return rc;
+  }
+  return DINVK_OK;
+}
+
+// ---- stencil kernels -----------------------------------------------------------------------------------------------
+
+// f(i, h, w) for every pixel i of a (planes, H, W) stack of n pixels, grid-stride
+template <class F>
+__device__ __forceinline__ void for_each_pixel(int H, int W, long long n, F&& f) {
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const long long plane = i / ((long long)H * W);
+    const int hw = (int)(i - plane * H * W);
+    f(i, hw / W, hw % W);
+  }
 }
 
 __global__ void __launch_bounds__(256) nabla_kernel(const float* __restrict__ x, float2* __restrict__ g, int H, int W, long long n) {
-  const long long stride = (long long)gridDim.x * blockDim.x;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-    const long long plane = i / ((long long)H * W);
-    const int hw = (int)(i - plane * H * W), h = hw / W, w = hw % W;
-    g[i] = nabla_at(x + plane * H * W, h, w, H, W);
-  }
+  for_each_pixel(H, W, n, [&](long long i, int h, int w) { g[i] = nabla(around(x, i, W), h, w, H, W); });
 }
 
 __global__ void __launch_bounds__(256) nabla_adjoint_kernel(const float2* __restrict__ g, float* __restrict__ x, int H, int W, long long n) {
-  const long long stride = (long long)gridDim.x * blockDim.x;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-    const long long plane = i / ((long long)H * W);
-    const int hw = (int)(i - plane * H * W), h = hw / W, w = hw % W;
-    const float2* gp = g + plane * H * W;
-    x[i] = adjoint_at([&](int hh, int ww) { return gp[(long long)hh * W + ww]; }, h, w, H, W);
-  }
+  for_each_pixel(H, W, n, [&](long long i, int h, int w) { x[i] = nabla_adjoint(around(g, i, W), h, w, H, W); });
 }
 
-// TGVDenoiser.epsilon (tgv.py:229-270): (…,2) -> (…,4), component 2i + j = backward difference of field component i along
-// axis j (0: H, 1: W), stored at the upper index; zero on the first row / column
 __global__ void __launch_bounds__(256) epsilon_kernel(const float2* __restrict__ f, float4* __restrict__ g, int H, int W, long long n) {
-  const long long stride = (long long)gridDim.x * blockDim.x;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-    const long long plane = i / ((long long)H * W);
-    const int hw = (int)(i - plane * H * W), h = hw / W, w = hw % W;
-    const float2 v = f[i];
-    float4 e = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (h > 0) {
-      const float2 a = f[i - W];
-      e.x = __fsub_rn(v.x, a.x);
-      e.z = __fsub_rn(v.y, a.y);
-    }
-    if (w > 0) {
-      const float2 a = f[i - 1];
-      e.y = __fsub_rn(v.x, a.x);
-      e.w = __fsub_rn(v.y, a.y);
-    }
-    g[i] = e;
-  }
+  for_each_pixel(H, W, n, [&](long long i, int h, int w) { g[i] = epsilon(around(f, i, W), h, w); });
 }
 
-// TGVDenoiser.epsilon_adjoint (tgv.py:272-312): (…,4) -> (…,2), each component in the reference's order of updates
 __global__ void __launch_bounds__(256) epsilon_adjoint_kernel(const float4* __restrict__ g, float2* __restrict__ f, int H, int W,
                                                               long long n) {
-  const long long stride = (long long)gridDim.x * blockDim.x;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-    const long long plane = i / ((long long)H * W);
-    const int hw = (int)(i - plane * H * W), h = hw / W, w = hw % W;
-    const float4 u = g[i];
-    float a0 = 0.f, a1 = 0.f;
-    if (h < H - 1) {
-      const float4 d = g[i + W];
-      a0 = __fsub_rn(a0, d.x);
-      a1 = __fsub_rn(a1, d.z);
-    }
-    if (h > 0) {
-      a0 = __fadd_rn(a0, u.x);
-      a1 = __fadd_rn(a1, u.z);
-    }
-    if (w < W - 1) {
-      const float4 e = g[i + 1];
-      a0 = __fsub_rn(a0, e.y);
-      a1 = __fsub_rn(a1, e.w);
-    }
-    if (w > 0) {
-      a0 = __fadd_rn(a0, u.y);
-      a1 = __fadd_rn(a1, u.w);
-    }
-    f[i] = make_float2(a0, a1);
-  }
+  for_each_pixel(H, W, n, [&](long long i, int h, int w) { f[i] = epsilon_adjoint(around(g, i, W), h, w, H, W); });
 }
 
 // TVPrior.grad (prior.py:544-572): nabla_adjoint(Dx / |Dx|), 0 where |Dx| = 0
 __global__ void __launch_bounds__(256) tv_grad_kernel(const float* __restrict__ x, float* __restrict__ out, int H, int W, long long n) {
-  const long long stride = (long long)gridDim.x * blockDim.x;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-    const long long plane = i / ((long long)H * W);
-    const int hw = (int)(i - plane * H * W), h = hw / W, w = hw % W;
-    const float* xp = x + plane * H * W;
-    out[i] = adjoint_at([&](int hh, int ww) {
-      const float2 d = nabla_at(xp, hh, ww, H, W);
+  for_each_pixel(H, W, n, [&](long long i, int h, int w) {
+    out[i] = nabla_adjoint([&](int dh, int dw) {
+      const float2 d = nabla(around(x, i + (long long)dh * W + dw, W), h + dh, w + dw, H, W);
       const float nrm = sqrtf(__fmaf_rn(d.y, d.y, __fmul_rn(d.x, d.x)));
       return nrm > 0.f ? make_float2(d.x / nrm, d.y / nrm) : make_float2(0.f, 0.f);
     }, h, w, H, W);
-  }
+  });
 }
 
 __device__ __forceinline__ double block_sum(double v, double* part) {
@@ -677,7 +649,7 @@ __global__ void __launch_bounds__(256) tv_fn_partial_kernel(double* __restrict__
   for (long long i = (long long)ch * blockDim.x + threadIdx.x; i < n_per; i += (long long)chunks * blockDim.x) {
     const int c = (int)(i / ((long long)H * W));
     const int hw = (int)(i - (long long)c * H * W);
-    const float2 d = nabla_at(x + (long long)b * n_per + (long long)c * H * W, hw / W, hw % W, H, W);
+    const float2 d = nabla(around(x, (long long)b * n_per + i, W), hw / W, hw % W, H, W);
     acc += mode == 0 ? (double)sqrtf(__fadd_rn(__fmul_rn(d.x, d.x), __fmul_rn(d.y, d.y))) : (double)fabsf(d.x) + (double)fabsf(d.y);
   }
   const double r = block_sum(acc, part);
@@ -705,75 +677,30 @@ static int fn_chunks(int B, long long n_per) {
   return (int)std::max(1LL, std::min(want, cap));
 }
 
-static int tiles(int n) { return (n + T - 1) / T; }
-
 }  // namespace tv
 }  // namespace dinvk
 
 using namespace dinvk;
 
 extern "C" int dinvk_tv_block(int* tile, int* iters) {
-  if (tile) *tile = tv::T;
-  if (iters) *iters = tv::K;
+  if (tile) *tile = tv::TvTile::T;
+  if (iters) *iters = tv::TvTile::K;
   return DINVK_OK;
 }
 
-extern "C" size_t dinvk_tv_prox_workspace_bytes(int B, int C, int H, int W) {
-  const size_t n_cta = (size_t)std::max(B, 0) * std::max(C, 0) * tv::tiles(std::max(H, 1)) * tv::tiles(std::max(W, 1));
-  return tv::CTRL_BYTES + sizeof(double) * 2 * tv::K * std::max<size_t>(n_cta, 1);
-}
+extern "C" size_t dinvk_tv_prox_workspace_bytes(int B, int C, int H, int W) { return tv::workspace_bytes<tv::TvTile>(B, C, H, W); }
 
 extern "C" int dinvk_tv_prox(const float* y, float* x2_a, float* u2_a, float* x2_b, float* u2_b, const float* lambd, int B, int C,
                              int H, int W, int n_it_max, float crit, double tau, double rho, int mode, int first, int n_launch,
                              void* workspace, size_t workspace_bytes, void* stream) {
   DINVK_CHECK_ARG(y && x2_a && u2_a && x2_b && u2_b && lambd && workspace, "dinvk_tv_prox: null pointer");
-  DINVK_CHECK_ARG(B >= 0 && C >= 0 && H > 0 && W > 0 && n_it_max >= 0 && n_launch >= 0, "dinvk_tv_prox: bad shape");
   DINVK_CHECK_ARG(mode == 0 || mode == 1, "dinvk_tv_prox: mode must be 0 (TV) or 1 (TV-L1)");
-  DINVK_CHECK_ARG((reinterpret_cast<uintptr_t>(u2_a) & 7) == 0 && (reinterpret_cast<uintptr_t>(u2_b) & 7) == 0 &&
-                      (reinterpret_cast<uintptr_t>(workspace) & 7) == 0,
-                  "dinvk_tv_prox: u2 buffers and workspace must be 8-byte aligned");
-  if (workspace_bytes < dinvk_tv_prox_workspace_bytes(B, C, H, W))
-    return set_error(DINVK_EWORKSPACE, "dinvk_tv_prox: workspace too small");
-  const long long n_cta = (long long)B * C * tv::tiles(H) * tv::tiles(W);
-  DINVK_CHECK_ARG(n_cta < (1LL << 31), "dinvk_tv_prox: too many tiles");
-  tv::Params p;
-  p.y = y;
-  p.x2[0] = x2_a;
-  p.x2[1] = x2_b;
-  p.u2[0] = reinterpret_cast<float2*>(u2_a);
-  p.u2[1] = reinterpret_cast<float2*>(u2_b);
-  p.lambd = lambd;
-  p.ctrl = reinterpret_cast<tv::Ctrl*>(workspace);
-  p.slots = reinterpret_cast<double*>(static_cast<char*>(workspace) + tv::CTRL_BYTES);
-  p.C = C;
-  p.H = H;
-  p.W = W;
-  p.tiles_x = tv::tiles(W);
-  p.tiles_per_plane = tv::tiles(H) * tv::tiles(W);
-  p.n_cta = (int)n_cta;
-  p.n_it_max = n_it_max;
-  p.mode = mode;
-  p.crit = crit;
-  // the reference's constants: python doubles rounded once to fp32 by torch (tv.py:119-121, 72)
-  p.tau = (float)tau;
-  p.one_plus_tau = (float)(1.0 + tau);
-  p.sigma = (float)(1.0 / tau / 8.0);  // 1 / tau / 2^(ndim - 1) with ndim = 4 (tv.py:119-121)
-  p.rho = (float)rho;
-  if (first) {
-    cudaError_t e = cudaMemsetAsync(workspace, 0, tv::CTRL_BYTES, (cudaStream_t)stream);
-    if (e != cudaSuccess) return set_error(DINVK_ECUDA, "dinvk_tv_prox: memset: %s", cudaGetErrorString(e));
-  }
-  if (n_cta == 0) return DINVK_OK;
-  int rc;
-#ifndef DINVK_EMUL
-  // opt in even at exactly 48 KB of dynamic shared memory: the static reduction buffers come on top of it
-  if ((rc = raise_smem_limit(reinterpret_cast<const void*>(tv::tv_cp_kernel), tv::SMEM))) return rc;
-#endif
-  for (int l = 0; l < n_launch; ++l) {
-    DINVK_LAUNCH(tv::tv_cp_kernel, dim3((unsigned)n_cta), dim3(tv::NT), tv::SMEM, stream, p);
-    if ((rc = DINVK_POST_LAUNCH())) return rc;
-  }
-  return DINVK_OK;
+  DINVK_CHECK_ARG((reinterpret_cast<uintptr_t>(u2_a) & 7) == 0 && (reinterpret_cast<uintptr_t>(u2_b) & 7) == 0,
+                  "dinvk_tv_prox: u2 buffers must be 8-byte aligned");
+  tv::TvParams p{{}, y, {x2_a, x2_b}, {reinterpret_cast<float2*>(u2_a), reinterpret_cast<float2*>(u2_b)}, lambd, mode};
+  // sigma = 1 / tau / 2^(ndim - 1) with ndim = 4 (tv.py:119-121)
+  return tv::run_cp<tv::TvTile>("dinvk_tv_prox", tv::tv_cp_kernel, tv::TV_SMEM, p, B, C, H, W, n_it_max, crit, tau, 1.0 / tau / 8.0,
+                                rho, first, n_launch, workspace, workspace_bytes, stream);
 }
 
 extern "C" int dinvk_tv_stencil(int op, const float* in, float* out, int B, int C, int H, int W, void* stream) {
@@ -803,69 +730,26 @@ extern "C" int dinvk_tv_stencil(int op, const float* in, float* out, int B, int 
 }
 
 extern "C" int dinvk_tgv_block(int* tile, int* iters) {
-  if (tile) *tile = tgv::T;
-  if (iters) *iters = tgv::K;
+  if (tile) *tile = tv::TgvTile::T;
+  if (iters) *iters = tv::TgvTile::K;
   return DINVK_OK;
 }
 
-extern "C" size_t dinvk_tgv_prox_workspace_bytes(int B, int C, int H, int W) {
-  const size_t n_cta = (size_t)std::max(B, 0) * std::max(C, 0) * tgv::tiles(std::max(H, 1)) * tgv::tiles(std::max(W, 1));
-  return tv::CTRL_BYTES + sizeof(double) * 2 * tgv::K * std::max<size_t>(n_cta, 1);
-}
+extern "C" size_t dinvk_tgv_prox_workspace_bytes(int B, int C, int H, int W) { return tv::workspace_bytes<tv::TgvTile>(B, C, H, W); }
 
 extern "C" int dinvk_tgv_prox(const float* y, float* x2_a, float* r2_a, float* u2_a, float* x2_b, float* r2_b, float* u2_b,
                               const float* tl1, const float* l2, int B, int C, int H, int W, int n_it_max, float crit, double tau,
                               double rho, int first, int n_launch, void* workspace, size_t workspace_bytes, void* stream) {
   DINVK_CHECK_ARG(y && x2_a && r2_a && u2_a && x2_b && r2_b && u2_b && tl1 && l2 && workspace, "dinvk_tgv_prox: null pointer");
-  DINVK_CHECK_ARG(B >= 0 && C >= 0 && H > 0 && W > 0 && n_it_max >= 0 && n_launch >= 0, "dinvk_tgv_prox: bad shape");
   DINVK_CHECK_ARG((reinterpret_cast<uintptr_t>(u2_a) & 15) == 0 && (reinterpret_cast<uintptr_t>(u2_b) & 15) == 0,
                   "dinvk_tgv_prox: u2 buffers must be 16-byte aligned");
-  DINVK_CHECK_ARG((reinterpret_cast<uintptr_t>(r2_a) & 7) == 0 && (reinterpret_cast<uintptr_t>(r2_b) & 7) == 0 &&
-                      (reinterpret_cast<uintptr_t>(workspace) & 7) == 0,
-                  "dinvk_tgv_prox: r2 buffers and workspace must be 8-byte aligned");
-  if (workspace_bytes < dinvk_tgv_prox_workspace_bytes(B, C, H, W))
-    return set_error(DINVK_EWORKSPACE, "dinvk_tgv_prox: workspace too small");
-  const long long n_cta = (long long)B * C * tgv::tiles(H) * tgv::tiles(W);
-  DINVK_CHECK_ARG(n_cta < (1LL << 31), "dinvk_tgv_prox: too many tiles");
-  tgv::Params p;
-  p.y = y;
-  p.x2[0] = x2_a;
-  p.x2[1] = x2_b;
-  p.r2[0] = reinterpret_cast<float2*>(r2_a);
-  p.r2[1] = reinterpret_cast<float2*>(r2_b);
-  p.u2[0] = reinterpret_cast<float4*>(u2_a);
-  p.u2[1] = reinterpret_cast<float4*>(u2_b);
-  p.tl1 = tl1;
-  p.l2 = l2;
-  p.ctrl = reinterpret_cast<tv::Ctrl*>(workspace);
-  p.slots = reinterpret_cast<double*>(static_cast<char*>(workspace) + tv::CTRL_BYTES);
-  p.C = C;
-  p.H = H;
-  p.W = W;
-  p.tiles_x = tgv::tiles(W);
-  p.tiles_per_plane = tgv::tiles(H) * tgv::tiles(W);
-  p.n_cta = (int)n_cta;
-  p.n_it_max = n_it_max;
-  p.crit = crit;
-  // the reference's constants: python doubles rounded once to fp32 by torch (tgv.py:63-65, 74, 122)
-  p.tau = (float)tau;
-  p.one_plus_tau = (float)(1.0 + tau);
-  p.sigma = (float)(1.0 / tau / 72.0);  // 1 / tau / 72 in 2-D (tgv.py:121-122)
-  p.rho = (float)rho;
-  if (first) {
-    cudaError_t e = cudaMemsetAsync(workspace, 0, tv::CTRL_BYTES, (cudaStream_t)stream);
-    if (e != cudaSuccess) return set_error(DINVK_ECUDA, "dinvk_tgv_prox: memset: %s", cudaGetErrorString(e));
-  }
-  if (n_cta == 0) return DINVK_OK;
-  int rc;
-#ifndef DINVK_EMUL
-  if ((rc = raise_smem_limit(reinterpret_cast<const void*>(tgv::tgv_cp_kernel), tgv::SMEM))) return rc;
-#endif
-  for (int l = 0; l < n_launch; ++l) {
-    DINVK_LAUNCH(tgv::tgv_cp_kernel, dim3((unsigned)n_cta), dim3(tgv::NT), tgv::SMEM, stream, p);
-    if ((rc = DINVK_POST_LAUNCH())) return rc;
-  }
-  return DINVK_OK;
+  DINVK_CHECK_ARG((reinterpret_cast<uintptr_t>(r2_a) & 7) == 0 && (reinterpret_cast<uintptr_t>(r2_b) & 7) == 0,
+                  "dinvk_tgv_prox: r2 buffers must be 8-byte aligned");
+  tv::TgvParams p{{}, y, {x2_a, x2_b}, {reinterpret_cast<float2*>(r2_a), reinterpret_cast<float2*>(r2_b)},
+                  {reinterpret_cast<float4*>(u2_a), reinterpret_cast<float4*>(u2_b)}, tl1, l2};
+  // sigma = 1 / tau / 72 in 2-D (tgv.py:121-122)
+  return tv::run_cp<tv::TgvTile>("dinvk_tgv_prox", tv::tgv_cp_kernel, tv::TGV_SMEM, p, B, C, H, W, n_it_max, crit, tau,
+                                 1.0 / tau / 72.0, rho, first, n_launch, workspace, workspace_bytes, stream);
 }
 
 extern "C" size_t dinvk_tv_fn_workspace_bytes(int B, int C, int H, int W) {

@@ -643,7 +643,7 @@ def tv_block(lib=None) -> tuple[int, int]:
 
 
 def tv_drive(launch, read_ctrl, n_it_max: int, iters_per_launch: int, check_every: int) -> dict:
-    """Host loop of the TV prox, shared with the emulation tests.
+    """Host loop of the TV and TGV proxes.
 
     `launch(first, n)` enqueues n iteration blocks; `read_ctrl()` synchronises and returns the control block as a dict.
     Issues ceil(n_it_max / K) blocks, reading the control block every `check_every` launches and after the last one;
@@ -669,6 +669,33 @@ def tv_drive(launch, read_ctrl, n_it_max: int, iters_per_launch: int, check_ever
     return ctrl
 
 
+def read_ctrl(ws: torch.Tensor) -> dict:
+    """the control block at the head of a TV / TGV prox workspace (a byte tensor), as a dict; synchronises"""
+    return dict(zip(TV_CTRL_FIELDS, ws[:4 * len(TV_CTRL_FIELDS)].view(torch.int32).tolist()))
+
+
+def _cp_prox(lib, stream, call, state, nb: int, K: int, n_it_max: int, check_every: int, stats: Optional[dict] = None,
+             fill: Optional[float] = None):
+    """Run one TV / TGV prox from `state`, a list of state tensors, and return (state after the solve, control block).
+
+    `call(*a, *b, first, n, ws, nb, stream)` calls the library's entry point with the pointers of the ping-pong state
+    buffers a and b.  a starts as a copy of `state`; b is scratch, left uninitialised unless `fill` is given.  A replay
+    needs its launch's input intact, which is why the buffers alternate.  nb is the workspace size in bytes, K the
+    iterations per launch.  Works on CPU tensors with a None stream.
+    """
+    a = [t.float().clone(memory_format=torch.contiguous_format) for t in state]
+    b = [torch.empty_like(t) if fill is None else torch.full_like(t, fill) for t in a]
+    ws = torch.empty(nb, dtype=torch.uint8, device=a[0].device)  # per call: the control block is the solve's state
+
+    def launch(first, n):
+        check(call(*map(_p, a), *map(_p, b), int(first), n, _p(ws), nb, stream), lib)
+
+    ctrl = tv_drive(launch, lambda: read_ctrl(ws), n_it_max if a[0].numel() else 0, K, check_every)
+    if stats is not None:
+        stats.update(launches=ctrl["launches"], syncs=ctrl["syncs"], converged=bool(ctrl["conv_j1"]))
+    return (b if ctrl["cur"] else a), ctrl
+
+
 def tv_prox(y: torch.Tensor, lambd: torch.Tensor, x2: torch.Tensor, u2: torch.Tensor, l1: bool = False, tau: float = 0.01,
             rho: float = 1.99, n_it_max: int = 1000, crit: float = 1e-5, check_every: int = 16, stats: Optional[dict] = None):
     """TVDenoiser / TVL1Denoiser iterations from the state (x2 (B,C,H,W), u2 (B,C,H,W,2)); lambd (B,) on the device.
@@ -683,31 +710,13 @@ def tv_prox(y: torch.Tensor, lambd: torch.Tensor, x2: torch.Tensor, u2: torch.Te
     B, C, H, W = y.shape
     if lambd.numel() != B:
         raise DinvkError(f"lambd must hold one value per sample: {lambd.numel()} values for a batch of {B}")
-    # ping-pong state buffers: (a) the start state, (b) scratch; a replay needs its launch's input intact
-    xa, ua = x2.float().clone(memory_format=torch.contiguous_format), u2.float().clone(memory_format=torch.contiguous_format)
-    xb, ub = torch.empty_like(xa), torch.empty_like(ua)
     lib = get_lib()
-    nb = lib.dinvk_tv_prox_workspace_bytes(B, C, H, W)
-    ws = torch.empty(nb, dtype=torch.uint8, device=dev)  # per call: the control block is the solve's state
-    stream = _stream(dev)
-    _, K = tv_block(lib)
-
-    def launch(first, n):
-        check(lib.dinvk_tv_prox(_p(y), _p(xa), _p(ua), _p(xb), _p(ub), _p(lambd), B, C, H, W, int(n_it_max), float(crit),
-                                float(tau), float(rho), int(l1), int(first), n, _p(ws), nb, stream))
-
-    def read_ctrl():
-        return dict(zip(TV_CTRL_FIELDS, ws[:24].view(torch.int32).tolist()))
-
-    if n_it_max <= 0 or y.numel() == 0:
-        ctrl = {"cur": 0, "launches": 0, "syncs": 0}
-        iters = torch.zeros((), dtype=torch.int32, device=dev)
-    else:
-        ctrl = tv_drive(launch, read_ctrl, n_it_max, K, check_every)
-        iters = torch.full((), ctrl["it_done"], dtype=torch.int32, device=dev)
-    if stats is not None:
-        stats.update(launches=ctrl["launches"], syncs=ctrl["syncs"], converged=bool(ctrl.get("conv_j1", 0)))
-    return (xb, ub, iters) if ctrl["cur"] else (xa, ua, iters)
+    (x, u), ctrl = _cp_prox(
+        lib, _stream(dev),
+        lambda xa, ua, xb, ub, *run: lib.dinvk_tv_prox(_p(y), xa, ua, xb, ub, _p(lambd), B, C, H, W, int(n_it_max), float(crit),
+                                                       float(tau), float(rho), int(l1), *run),
+        [x2, u2], lib.dinvk_tv_prox_workspace_bytes(B, C, H, W), tv_block(lib)[1], n_it_max, check_every, stats)
+    return x, u, torch.full((), ctrl["it_done"], dtype=torch.int32, device=dev)
 
 
 def _tv_shape(x: torch.Tensor, what: str) -> None:
@@ -793,31 +802,13 @@ def tgv_prox(y: torch.Tensor, tl1: torch.Tensor, l2: torch.Tensor, x2: torch.Ten
         raise DinvkError(f"tl1 and l2 must hold one value per sample: {tl1.numel()}, {l2.numel()} values for a batch of {B}")
     if r2.shape != (B, C, H, W, 2) or u2.shape != (B, C, H, W, 4) or x2.shape != y.shape:
         raise DinvkError(f"TGV state shapes {tuple(x2.shape)}, {tuple(r2.shape)}, {tuple(u2.shape)} do not match y {tuple(y.shape)}")
-    # ping-pong state buffers: (a) the start state, (b) scratch; a replay needs its launch's input intact
-    xa, ra, ua = (t.float().clone(memory_format=torch.contiguous_format) for t in (x2, r2, u2))
-    xb, rb, ub = torch.empty_like(xa), torch.empty_like(ra), torch.empty_like(ua)
     lib = get_lib()
-    nb = lib.dinvk_tgv_prox_workspace_bytes(B, C, H, W)
-    ws = torch.empty(nb, dtype=torch.uint8, device=dev)  # per call: the control block is the solve's state
-    stream = _stream(dev)
-    _, K = tgv_block(lib)
-
-    def launch(first, n):
-        check(lib.dinvk_tgv_prox(_p(y), _p(xa), _p(ra), _p(ua), _p(xb), _p(rb), _p(ub), _p(tl1), _p(l2), B, C, H, W,
-                                 int(n_it_max), float(crit), float(tau), float(rho), int(first), n, _p(ws), nb, stream))
-
-    def read_ctrl():
-        return dict(zip(TV_CTRL_FIELDS, ws[:24].view(torch.int32).tolist()))
-
-    if n_it_max <= 0 or y.numel() == 0:
-        ctrl = {"cur": 0, "launches": 0, "syncs": 0}
-        iters = torch.zeros((), dtype=torch.int32, device=dev)
-    else:
-        ctrl = tv_drive(launch, read_ctrl, n_it_max, K, check_every)
-        iters = torch.full((), ctrl["it_done"], dtype=torch.int32, device=dev)
-    if stats is not None:
-        stats.update(launches=ctrl["launches"], syncs=ctrl["syncs"], converged=bool(ctrl.get("conv_j1", 0)))
-    return (xb, rb, ub, iters) if ctrl["cur"] else (xa, ra, ua, iters)
+    (x, r, u), ctrl = _cp_prox(
+        lib, _stream(dev),
+        lambda xa, ra, ua, xb, rb, ub, *run: lib.dinvk_tgv_prox(_p(y), xa, ra, ua, xb, rb, ub, _p(tl1), _p(l2), B, C, H, W,
+                                                                int(n_it_max), float(crit), float(tau), float(rho), *run),
+        [x2, r2, u2], lib.dinvk_tgv_prox_workspace_bytes(B, C, H, W), tgv_block(lib)[1], n_it_max, check_every, stats)
+    return x, r, u, torch.full((), ctrl["it_done"], dtype=torch.int32, device=dev)
 
 
 def tgv_epsilon(f: torch.Tensor) -> torch.Tensor:

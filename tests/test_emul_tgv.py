@@ -1,8 +1,8 @@
 """The TGV kernels (deepinv_b200/csrc/tv.cu) run on the host through the emulation, against the torch oracle
 (tests/tgv_oracle.py).
 
-The prox is driven by the package's own host loop (`ops.tv_drive`).  Covered: tiles at every border with H and W not
-multiples of the tile edge and B*C > 1, n_it_max not a multiple of the iterations per launch K, warm restart, the break
+The prox is driven by the package's own host side (`ops._cp_prox`, `ops.tv_drive`).  Covered: tiles at every border with H
+and W not multiples of the tile edge and B*C > 1, n_it_max not a multiple of the iterations per launch K, warm restart, the break
 test passing at sub-iterations 0, K - 2 and K - 1 of a launch (the replay must be bitwise the run stopped at that
 iteration), ths = 0, the epsilon stencils and their adjointness, and two builds with a different tile edge and K giving
 the same bits.
@@ -15,30 +15,17 @@ import pytest
 import torch
 
 sys.path.insert(0, str(Path(__file__).resolve().parent))
-sys.path.insert(0, str(Path(__file__).resolve().parent / "emul"))
 import tgv_oracle as O  # noqa: E402
+from emul_tv_util import _p, image, lib, rel  # noqa: E402
 
-from deepinv_b200 import _ffi, ops  # noqa: E402
+from deepinv_b200 import ops  # noqa: E402
 
-_libs = {}
 ALT = (20, 3)  # a second build: another tile edge and K, R = 32
-
-
-def lib(tk=None):
-    if tk not in _libs:
-        from build_emul_tgv import build
-
-        _libs[tk] = _ffi.bind(C.CDLL(str(build(*(tk or (None, None))))), required=False)
-    return _libs[tk]
-
-
-def _p(t):
-    return C.c_void_p(t.data_ptr())
 
 
 def block(tk=None):
     t, k = C.c_int(0), C.c_int(0)
-    lib(tk).dinvk_tgv_block(C.byref(t), C.byref(k))
+    lib(tgv=tk).dinvk_tgv_block(C.byref(t), C.byref(k))
     return t.value, k.value
 
 
@@ -48,38 +35,18 @@ def constants(lam, B, tau=0.01):
 
 
 def prox_emul(y, lam, n_it_max=12, crit=0.0, x2=None, r2=None, u2=None, rho=1.99, check_every=2, tk=None):
-    L = lib(tk)
+    L = lib(tgv=tk)
     B, Cc, H, W = y.shape
     y = y.float().contiguous()
     tl1, l2 = constants(lam, B)
-    xa = (y if x2 is None else x2).clone()
-    ra = torch.zeros(B, Cc, H, W, 2) if r2 is None else r2.clone()
-    ua = torch.zeros(B, Cc, H, W, 4) if u2 is None else u2.clone()
-    xb, rb, ub = (torch.full_like(t, float("nan")) for t in (xa, ra, ua))
-    nb = L.dinvk_tgv_prox_workspace_bytes(B, Cc, H, W)
-    ws = torch.zeros(nb // 8 + 1, dtype=torch.float64)
-
-    def launch(first, n):
-        rc = L.dinvk_tgv_prox(_p(y), _p(xa), _p(ra), _p(ua), _p(xb), _p(rb), _p(ub), _p(tl1), _p(l2), B, Cc, H, W, n_it_max, crit,
-                              0.01, rho, int(first), n, _p(ws), nb, None)
-        assert rc == 0, L.dinvk_last_error()
-
-    def read_ctrl():
-        return dict(zip(ops.TV_CTRL_FIELDS, ws[:3].view(torch.int32).tolist()))
-
-    ctrl = ops.tv_drive(launch, read_ctrl, n_it_max, block(tk)[1], check_every)
-    x, r, u = (xb, rb, ub) if ctrl["cur"] else (xa, ra, ua)
+    state = [y if x2 is None else x2, torch.zeros(B, Cc, H, W, 2) if r2 is None else r2,
+             torch.zeros(B, Cc, H, W, 4) if u2 is None else u2]
+    (x, r, u), ctrl = ops._cp_prox(
+        L, None,
+        lambda xa, ra, ua, xb, rb, ub, *run: L.dinvk_tgv_prox(_p(y), xa, ra, ua, xb, rb, ub, _p(tl1), _p(l2), B, Cc, H, W, n_it_max,
+                                                              crit, 0.01, rho, *run),
+        state, L.dinvk_tgv_prox_workspace_bytes(B, Cc, H, W), block(tk)[1], n_it_max, check_every, fill=float("nan"))
     return x, r, u, ctrl
-
-
-def rel(a, b):
-    return float((a.double() - b.double()).norm() / b.double().norm())
-
-
-def image(B, Cc, H, W, seed=0):
-    g = torch.Generator().manual_seed(seed)
-    base = torch.linspace(0, 1, W).expand(H, W) + torch.linspace(0, 0.5, H)[:, None]
-    return (base + 0.3 * torch.randn(B, Cc, H, W, generator=g)).float()
 
 
 def test_block_constants():
@@ -185,7 +152,7 @@ def test_tile_and_block_change_no_bit():
 def _stencil(op, x, out_shape, tk=None):
     out = torch.empty(out_shape)
     B, Cc, H, W = x.shape[:-1]
-    assert lib(tk).dinvk_tv_stencil(op, _p(x.contiguous()), _p(out), B, Cc, H, W, None) == 0
+    assert lib(tgv=tk).dinvk_tv_stencil(op, _p(x.contiguous()), _p(out), B, Cc, H, W, None) == 0
     return out
 
 

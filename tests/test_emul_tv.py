@@ -1,9 +1,9 @@
 """The TV kernels (deepinv_b200/csrc/tv.cu) run on the host through the emulation, against the torch oracle (tests/tv_oracle.py).
 
-The prox is driven by the package's own host loop (`ops.tv_drive`).  Covered: tiles at every border with H and W not
-multiples of the tile edge and B*C > 1, n_it_max not a multiple of the iterations per launch K, the break test passing
-at sub-iterations 0, K - 2 and K - 1 of a launch (the replay must be bitwise the run stopped at that iteration), warm
-restart, both dual projections, and the stencils.
+The prox is driven by the package's own host side (`ops._cp_prox`, `ops.tv_drive`).  Covered: tiles at every border with H
+and W not multiples of the tile edge and B*C > 1, n_it_max not a multiple of the iterations per launch K, the break test
+passing at sub-iterations 0, K - 2 and K - 1 of a launch (the replay must be bitwise the run stopped at that iteration),
+warm restart, both dual projections, the stencils, and two builds with a different tile edge and K giving the same bits.
 """
 import ctypes as C
 import sys
@@ -13,70 +13,38 @@ import pytest
 import torch
 
 sys.path.insert(0, str(Path(__file__).resolve().parent))
-sys.path.insert(0, str(Path(__file__).resolve().parent / "emul"))
 import tv_oracle as O  # noqa: E402
+from emul_tv_util import _p, image, lib, rel  # noqa: E402
 
-from deepinv_b200 import _ffi, ops  # noqa: E402
+from deepinv_b200 import ops  # noqa: E402
 
-_lib = None
-
-
-def lib():
-    global _lib
-    if _lib is None:
-        from build_emul_tv import build
-
-        _lib = _ffi.bind(C.CDLL(str(build())), required=False)
-    return _lib
+ALT = (20, 3)  # a second build: another tile edge and K, R = 26
 
 
-def _p(t):
-    return C.c_void_p(t.data_ptr())
-
-
-def prox_emul(y, lam, l1=False, n_it_max=20, crit=0.0, x2=None, u2=None, tau=0.01, rho=1.99, check_every=2):
-    L = lib()
+def prox_emul(y, lam, l1=False, n_it_max=20, crit=0.0, x2=None, u2=None, tau=0.01, rho=1.99, check_every=2, tk=None):
+    L = lib(tv=tk)
     B, Cc, H, W = y.shape
     y = y.float().contiguous()
     lam = torch.as_tensor(lam, dtype=torch.float32).expand(B).contiguous()
-    xa = (y if x2 is None else x2).clone()
-    ua = torch.zeros(B, Cc, H, W, 2) if u2 is None else u2.clone()
-    xb, ub = torch.full_like(xa, float("nan")), torch.full_like(ua, float("nan"))
-    nb = L.dinvk_tv_prox_workspace_bytes(B, Cc, H, W)
-    ws = torch.zeros(nb // 8 + 1, dtype=torch.float64)
-
-    def launch(first, n):
-        rc = L.dinvk_tv_prox(_p(y), _p(xa), _p(ua), _p(xb), _p(ub), _p(lam), B, Cc, H, W, n_it_max, crit, tau, rho, int(l1),
-                             int(first), n, _p(ws), nb, None)
-        assert rc == 0, L.dinvk_last_error()
-
-    def read_ctrl():
-        return dict(zip(ops.TV_CTRL_FIELDS, ws[:3].view(torch.int32).tolist()))
-
-    ctrl = ops.tv_drive(launch, read_ctrl, n_it_max, block()[1], check_every)
-    x, u = (xb, ub) if ctrl["cur"] else (xa, ua)
+    state = [y if x2 is None else x2, torch.zeros(B, Cc, H, W, 2) if u2 is None else u2]
+    (x, u), ctrl = ops._cp_prox(
+        L, None,
+        lambda xa, ua, xb, ub, *run: L.dinvk_tv_prox(_p(y), xa, ua, xb, ub, _p(lam), B, Cc, H, W, n_it_max, crit, tau, rho, int(l1),
+                                                     *run),
+        state, L.dinvk_tv_prox_workspace_bytes(B, Cc, H, W), block(tk)[1], n_it_max, check_every, fill=float("nan"))
     return x, u, ctrl
 
 
-def block():
+def block(tk=None):
     t, k = C.c_int(0), C.c_int(0)
-    lib().dinvk_tv_block(C.byref(t), C.byref(k))
+    lib(tv=tk).dinvk_tv_block(C.byref(t), C.byref(k))
     return t.value, k.value
-
-
-def rel(a, b):
-    return float((a.double() - b.double()).norm() / b.double().norm())
-
-
-def image(B, Cc, H, W, seed=0):
-    g = torch.Generator().manual_seed(seed)
-    base = torch.linspace(0, 1, W).expand(H, W) + torch.linspace(0, 0.5, H)[:, None]
-    return (base + 0.3 * torch.randn(B, Cc, H, W, generator=g)).float()
 
 
 def test_block_constants():
     T, K = block()
     assert T >= 16 and 2 <= K <= 16
+    assert block(ALT) == ALT
 
 
 @pytest.mark.parametrize("l1", [False, True])
@@ -158,6 +126,22 @@ def test_n_it_max_zero_issues_nothing():
     y = image(1, 1, 9, 9)
     x, u, ctrl = prox_emul(y, 0.1, n_it_max=0)
     assert ctrl["launches"] == 0 and torch.equal(x, y) and not u.any()
+
+
+def test_tile_and_block_change_no_bit():
+    y = image(2, 2, 71, 45, seed=6)
+    lam = torch.tensor([0.1, 0.4])
+    for l1 in (False, True):
+        a = prox_emul(y, lam, l1=l1, n_it_max=11)
+        b = prox_emul(y, lam, l1=l1, n_it_max=11, tk=ALT)
+        assert all(torch.equal(s, t) for s, t in zip(a[:2], b[:2]))
+    rels = []
+    O.tv_denoise(y, lam, rho=1.0, n_it_max=30, crit=0.0, rels=rels)
+    i, crit = _crit_breaking_at(rels, 1, 3, lo=5)  # inside a launch for K = 3; the default build breaks wherever i lands
+    a = prox_emul(y, lam, rho=1.0, n_it_max=30, crit=crit)
+    b = prox_emul(y, lam, rho=1.0, n_it_max=30, crit=crit, tk=ALT)
+    assert a[2]["it_done"] == b[2]["it_done"] == i + 1
+    assert all(torch.equal(s, t) for s, t in zip(a[:2], b[:2]))
 
 
 def _stencil(op, x, out_shape):
