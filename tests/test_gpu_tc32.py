@@ -197,6 +197,7 @@ def test_drunet_tc32_vs_oracle(precision, dev):
           f"tc32 vs oracle {rel_err(out, ref):.2e}")
     assert rel_err(out, ref) < 1e-5
     assert e_tc < 1e-5
+    assert e_simt < 1e-5  # the fp32 CUDA-core path (the one training differentiates) at the full width
 
 
 @pytest.mark.parametrize("precision", ["tc32", "tc32h"])

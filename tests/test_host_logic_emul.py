@@ -165,9 +165,11 @@ def test_dpir_schedule_toy_denoiser():
 
 
 # ---- SURVEY §8(f) item 2: training closure (backward kernels of the fp32 denoiser path) ---------------------------
-@pytest.mark.parametrize("kind,cin,cout,h,w", [(0, 5, 7, 11, 37), (0, 16, 40, 16, 64), (1, 6, 10, 8, 12), (2, 10, 6, 5, 7)])
+@pytest.mark.parametrize("kind,cin,cout,h,w", [(0, 5, 7, 11, 37), (0, 16, 40, 16, 64), (1, 6, 10, 8, 12), (2, 10, 6, 5, 7),
+                                               (1, 3, 5, 96, 98), (2, 5, 3, 48, 50)])
 def test_conv_backward_kernels(kind, cin, cout, h, w):
-    """data / weight / bias / residual / skip-input gradients of `ops.conv_f32_ag` == torch autograd of the same op"""
+    """data / weight / bias / residual / skip-input gradients of `ops.conv_f32_ag` == torch autograd of the same op.  The last
+    two shapes have M = 4704 and 4800 pixel rows: the 2x2 weight gradient then runs two 4096-row chunks, the second ragged."""
     import torch.nn.functional as F
     from conftest import rel_err
 
