@@ -17,7 +17,9 @@
 // One MMA "k step" on a 128-byte A row: steps 0,1 = the hi channels, steps 2,3 = the lo channels.
 //   hi step: A_hi x W_hi -> main,  A_hi x W_lo -> corr
 //   lo step: A_lo x W_hi -> corr
-// Every product is an N = 64 wgmma on a whole 32-register accumulator array: main = registers 0..31, corr = 32..63.
+// Every product is a wgmma on a whole accumulator array: per-tap kernel, N = 64 (pixels x output channels) with main =
+// registers 0..31 and corr = 32..63; slab kernel, N = 128 with the operands swapped (output channels x pixels), main = 0..63
+// and corr = 64..127.
 //
 // Kernels (persistent, one CTA per SM): consumer warpgroups issue wgmma (M = 64 rows each), drain, and run the epilogue
 // through a per-warp shared-memory staging buffer; one extra warp (warpgroup) is the TMA producer.
@@ -105,11 +107,30 @@ __device__ __forceinline__ void mma_block64(float* acc, uint32_t a, uint32_t a_h
   mma<F>(acc + 32, a + 4, a_hi, b, b_hi, 1u);            // lo, first half  x W_hi
   mma<F>(acc + 32, a + 6, a_hi, b + 2, b_hi, 1u);        // lo, second half x W_hi
 }
-// v[i] (row 16 * (warp % 4) + lane / 4 + 8 * ((i >> 1) & 1), column 8 * (i >> 2) + 2 * (lane % 4) + (i & 1)) += main + corr
 template <class F>
+__device__ __forceinline__ void mma128(float* d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi, uint32_t accumulate) {
+  if constexpr (F::ID == 0) tc::wgmma_tf32_n128(d, a_lo, a_hi, b_lo, b_hi, accumulate);
+  else tc::wgmma_f16_n128(d, a_lo, a_hi, b_lo, b_hi, accumulate);
+}
+// mma_block64 with the operands swapped: the weight rows [W_hi; W_lo] of one tap at descriptor w are A (M = 64 output
+// channels), 128 pixel rows [hi CH | lo CH] at descriptor x are B (N = 128):  acc[0, 64) main += W_hi X_hi,  acc[64, 128)
+// corr += W_lo X_hi + W_hi X_lo, in the order of mma_block64, so that every output element sees the same products in the
+// same order.  Six N = 128 wgmmas, each on a whole 64-register array.
+template <class F>
+__device__ __forceinline__ void mma_block128(float* acc, uint32_t w, uint32_t w_hi, uint32_t x, uint32_t x_hi, uint32_t fresh) {
+  mma128<F>(acc, w, w_hi, x, x_hi, fresh);                // W_hi x hi, first half  (main)
+  mma128<F>(acc + 64, w + 512, w_hi, x, x_hi, fresh);     // W_lo x hi, first half  (corr)
+  mma128<F>(acc, w + 2, w_hi, x + 2, x_hi, 1u);           // W_hi x hi, second half
+  mma128<F>(acc + 64, w + 514, w_hi, x + 2, x_hi, 1u);    // W_lo x hi, second half
+  mma128<F>(acc + 64, w, w_hi, x + 4, x_hi, 1u);          // W_hi x lo, first half
+  mma128<F>(acc + 64, w + 2, w_hi, x + 6, x_hi, 1u);      // W_hi x lo, second half
+}
+// v[i] += main + corr for the fragment of an N-column accumulator pair acc = [main (N / 2 registers); corr (N / 2)]:
+// v[i] is row 16 * (warp % 4) + lane / 4 + 8 * ((i >> 1) & 1), column 8 * (i >> 2) + 2 * (lane % 4) + (i & 1)
+template <class F, int N>
 __device__ __forceinline__ void drain(float* v, const float* acc) {
 #pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] += acc[i] + acc[32 + i] * F::CORR;
+  for (int i = 0; i < N / 2; ++i) v[i] += acc[i] + acc[N / 2 + i] * F::CORR;
 }
 
 // one warp's share of a consumed pipeline stage: the stage's `empty` barrier counts one arrival per consumer warp
@@ -253,6 +274,42 @@ __device__ __forceinline__ bool store_split16(typename F::elem* p, const float (
   return bad;
 }
 
+// the residual pieces [hi, lo] of res and res2 at element offset o (zero where absent, or if o < 0: outside the output)
+template <class F>
+__device__ __forceinline__ void load_res16(const Params& P, long long o, uint4 (&r1)[2], uint4 (&r2)[2]) {
+  using E = typename F::elem;
+  r1[0] = r1[1] = r2[0] = r2[1] = make_uint4(0u, 0u, 0u, 0u);
+  if (o < 0) return;
+  if (P.res) {
+    r1[0] = __ldg(reinterpret_cast<const uint4*>(static_cast<const E*>(P.res) + o));
+    r1[1] = __ldg(reinterpret_cast<const uint4*>(static_cast<const E*>(P.res) + o + F::CH));
+  }
+  if (P.res2) {
+    r2[0] = __ldg(reinterpret_cast<const uint4*>(static_cast<const E*>(P.res2) + o));
+    r2[1] = __ldg(reinterpret_cast<const uint4*>(static_cast<const E*>(P.res2) + o + F::CH));
+  }
+}
+// bias, ReLU, residuals and the split store of the K = 16 / EB channels a of one piece at element offset o of out; returns
+// true if a value left the format's range
+template <class F>
+__device__ __forceinline__ bool finish16(const Params& P, float (&a)[16 / F::EB], const float4 (&bv)[4 / F::EB], const uint4 (&r1)[2],
+                                         const uint4 (&r2)[2], long long o) {
+  constexpr int K = 16 / F::EB;
+  if (P.bias) {
+#pragma unroll
+    for (int k = 0; k < K / 4; ++k) {
+      a[4 * k] += bv[k].x; a[4 * k + 1] += bv[k].y; a[4 * k + 2] += bv[k].z; a[4 * k + 3] += bv[k].w;
+    }
+  }
+  if (P.relu) {
+#pragma unroll
+    for (int e = 0; e < K; ++e) a[e] = fmaxf(a[e], 0.f);
+  }
+  if (P.res) add_split16<F>(r1[0], r1[1], a);
+  if (P.res2) add_split16<F>(r2[0], r2[1], a);
+  return store_split16<F>(static_cast<typename F::elem*>(P.out) + o, a);
+}
+
 // float offset of (row r, 16-byte chunk k) in a warp's epilogue staging buffer (STG_WARP floats: 16 rows x 32 columns).  The
 // chunk is XORed with a function of the row so that the fragment writes (8 bytes per lane, rows lane / 4 and lane / 4 + 8)
 // and the row reads of both formats (16 bytes per lane, see epilogue) are free of bank conflicts.
@@ -267,7 +324,6 @@ __device__ __forceinline__ int stg_off(int r, int k) { return 32 * r + 4 * (k ^ 
 // c0 = output channel of column 0.
 template <class F, class PixelOf>
 __device__ __forceinline__ void epilogue(const Params& P, const float* v, float* stg, PixelOf pixel_of, int c0) {
-  using E = typename F::elem;
   constexpr int K = 16 / F::EB, NP = 16 / K;   // channels per lane, rows per lane (one per pass)
   const int lane = threadIdx.x & 31, q = lane & 3;
   const int rl = F::ID == 0 ? lane >> 3 : lane & 7;   // the lane's row in pass 0 (rows of pass p: rl + K p)
@@ -286,19 +342,7 @@ __device__ __forceinline__ void epilogue(const Params& P, const float* v, float*
 #pragma unroll
     for (int k = 0; k < K / 4; ++k) bv[k] = P.bias ? __ldg(reinterpret_cast<const float4*>(P.bias + c) + k) : make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
-    for (int p = 0; p < NP; ++p) {
-      r1[p][0] = r1[p][1] = r2[p][0] = r2[p][1] = make_uint4(0u, 0u, 0u, 0u);
-      if (pix[p] < 0) continue;
-      const long long o = pix[p] * P.Cout * 2 + oc;
-      if (P.res) {
-        r1[p][0] = __ldg(reinterpret_cast<const uint4*>(static_cast<const E*>(P.res) + o));
-        r1[p][1] = __ldg(reinterpret_cast<const uint4*>(static_cast<const E*>(P.res) + o + F::CH));
-      }
-      if (P.res2) {
-        r2[p][0] = __ldg(reinterpret_cast<const uint4*>(static_cast<const E*>(P.res2) + o));
-        r2[p][1] = __ldg(reinterpret_cast<const uint4*>(static_cast<const E*>(P.res2) + o + F::CH));
-      }
-    }
+    for (int p = 0; p < NP; ++p) load_res16<F>(P, pix[p] < 0 ? -1 : pix[p] * P.Cout * 2 + oc, r1[p], r2[p]);
     __syncwarp();
 #pragma unroll
     for (int j = 0; j < 4; ++j)
@@ -317,19 +361,61 @@ __device__ __forceinline__ void epilogue(const Params& P, const float* v, float*
         const float4 s = *reinterpret_cast<const float4*>(stg + stg_off(rl + K * p, K / 4 * cl + k));
         a[4 * k] = s.x; a[4 * k + 1] = s.y; a[4 * k + 2] = s.z; a[4 * k + 3] = s.w;
       }
-      if (P.bias) {
+      bad |= finish16<F>(P, a, bv, r1[p], r2[p], pix[p] * P.Cout * 2 + oc);
+    }
+  }
+  if (bad && P.flag) atomicOr(P.flag, 1);
+}
+
+// float offset of (output channel r, pixel n) in a warp's staging buffer for the slab kernel's transposed fragment (16
+// channels x 32 pixels).  Bits 3-4 of the pixel are XORed with the channel's bits 0-1 and 2-3, so that the fragment writes
+// (8 bytes per lane: channels lane / 4 (+ 8), pixels 2 (lane % 4) + 8 j) and the per-pixel reads of both formats (4 bytes
+// per lane, see epilogue_t) are free of bank conflicts.
+__device__ __forceinline__ int stg_off_t(int r, int n) { return 32 * r + (n ^ (8 * ((r ^ (r >> 2)) & 3))); }
+
+// epilogue of the slab kernel's drained sums v (see drain<F, 128>): the fragment of an m64 x n128 wgmma with the output
+// channels as rows and the pixels as columns; each warp owns its 16 output channels c0 .. c0 + 15 of 128 pixels.  The
+// fragment goes through the warp's staging buffer 32 pixels at a time.  Read back, a lane owns the K = 16 / EB channels of
+// one pixel whose hi words are one 16-byte piece, as in epilogue: fp16, channels 8 (lane % 2) .. of pixel lane / 2 (+ 16);
+// tf32, channels 4 (lane % 4) .. of pixel lane / 4 (+ 8, 16, 24).  The lanes of a pixel cover its 32 (fp16) or 64 (tf32)
+// bytes of hi words and of lo words, so every warp access covers whole 32-byte sectors.  pixel_of(n) = output pixel of
+// column n (0..127), or -1 outside the output.
+template <class F, class PixelOf>
+__device__ __forceinline__ void epilogue_t(const Params& P, const float* v, float* stg, PixelOf pixel_of, int c0) {
+  constexpr int K = 16 / F::EB, L = 16 / K, PP = 32 / L, NP = 32 / PP;   // channels per lane, lanes per pixel, pixels per pass, passes
+  const int lane = threadIdx.x & 31, q = lane & 3;
+  const int cl = lane % L, pl = lane / L;
+  const int c = c0 + K * cl;
+  const long long oc = (c / F::CH) * 2 * F::CH + (c % F::CH);   // element offset of the lane's channels in a pixel row
+  float4 bv[K / 4];
 #pragma unroll
-        for (int k = 0; k < K / 4; ++k) {
-          a[4 * k] += bv[k].x; a[4 * k + 1] += bv[k].y; a[4 * k + 2] += bv[k].z; a[4 * k + 3] += bv[k].w;
-        }
-      }
-      if (P.relu) {
+  for (int k = 0; k < K / 4; ++k) bv[k] = P.bias ? __ldg(reinterpret_cast<const float4*>(P.bias + c) + k) : make_float4(0.f, 0.f, 0.f, 0.f);
+  bool bad = false;
 #pragma unroll
-        for (int e = 0; e < K; ++e) a[e] = fmaxf(a[e], 0.f);
+  for (int chunk = 0; chunk < 4; ++chunk) {   // pixels 32 chunk .. 32 chunk + 31
+    long long pix[NP];
+    uint4 r1[NP][2], r2[NP][2];
+#pragma unroll
+    for (int p = 0; p < NP; ++p) {
+      pix[p] = pixel_of(32 * chunk + PP * p + pl);
+      load_res16<F>(P, pix[p] < 0 ? -1 : pix[p] * P.Cout * 2 + oc, r1[p], r2[p]);
+    }
+    __syncwarp();
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int i = 4 * (4 * chunk + j) + 2 * h;
+        *reinterpret_cast<float2*>(stg + stg_off_t((lane >> 2) + 8 * h, 8 * j + 2 * q)) = make_float2(v[i], v[i + 1]);
       }
-      if (P.res) add_split16<F>(r1[p][0], r1[p][1], a);
-      if (P.res2) add_split16<F>(r2[p][0], r2[p][1], a);
-      bad |= store_split16<F>(static_cast<E*>(P.out) + pix[p] * P.Cout * 2 + oc, a);
+    __syncwarp();
+#pragma unroll
+    for (int p = 0; p < NP; ++p) {
+      if (pix[p] < 0) continue;
+      float a[K];
+#pragma unroll
+      for (int e = 0; e < K; ++e) a[e] = stg[stg_off_t(K * cl + e, PP * p + pl)];
+      bad |= finish16<F>(P, a, bv, r1[p], r2[p], pix[p] * P.Cout * 2 + oc);
     }
   }
   if (bad && P.flag) atomicOr(P.flag, 1);
@@ -408,7 +494,7 @@ __global__ void __launch_bounds__(THREADS, 1) conv_tc32_kernel(const __grid_cons
         tc::reg_fence<64>(acc);
         release_stage(&empty_bar[s]);
         if (++in_win == P.win || kb == nk - 1) {
-          drain<F>(v, acc);
+          drain<F, 64>(v, acc);
           in_win = 0;
         }
         if (++s == STAGES) { s = 0; ph ^= 1; }
@@ -435,13 +521,15 @@ __global__ void __launch_bounds__(THREADS, 1) conv_tc32_kernel(const __grid_cons
 // 1024-byte periodic) of [hi | lo] rows into shared memory, and the nine taps are nine shifted wgmma descriptors into it
 // (start + (ky * SLAB_X + kx) * 128 B, stride between 8-row groups = one slab row); the 128-byte swizzle is a function of the
 // shared-memory address bits, so the shifted starts need no base offset.  A weight tile holds TWO taps of one channel block
-// ([tap even | tap odd] per row, rows = [W_hi; W_lo]) and feeds all four m64 blocks of the tile: 536 bytes from L2 per pixel
-// and channel block, where an 8 x 16 tile (two m64 blocks) needs 928.
+// ([tap even | tap odd] per row, rows = [W_hi; W_lo]) and feeds both consumer warpgroups: 536 bytes from L2 per pixel and
+// channel block, where an 8 x 16 tile needs 928.
 //
-// Consumer warpgroup g owns y-half g of the tile as TWO m64 blocks (x-halves 0 and 1, 8 x 8 pixels each): 2 x (64
-// accumulator + 32 drain) registers per thread, which a full producer warpgroup makes room for through setmaxnreg.  The MMAs
-// are N = 64 wgmmas (mma_block64), which ptxas keeps in flight back to back.  Every output element sees the same products in
-// the same order, with the same drains, as with one block per warpgroup.
+// The weights are the wgmma A operand (M = the 64 output channels of the N tile, the weight tile's rows as they are) and the
+// pixels the B operand: consumer warpgroup g owns x-half g of the tile, an 8-wide column of 16 slab rows = N = 128 pixels
+// (16 groups of 8 positions, one slab row apart).  Per tap, six N = 128 wgmmas (mma_block128) read 2 KB of weights and 4 KB
+// of pixels each, 96 bytes per tensor clock, where the N = 64 wgmmas with the pixels as A (two m64 blocks per warpgroup, each
+// re-reading the weight tile) read 128, the SM's whole shared-memory bandwidth.  A thread holds 64 main + 64 corr
+// accumulators and 64 drained floats, which a full producer warpgroup makes room for through setmaxnreg.
 // ---------------------------------------------------------------------------------------------------------------
 namespace slab {
 constexpr int TXP = 16, TYP = 16;                 // CTA pixel tile
@@ -453,7 +541,7 @@ constexpr int CONSUMER_WARPS = 8;                 // two warpgroups
 constexpr int SMEM_BYTES = A_STAGES * SLAB_BYTES + B_STAGES * WT_TILE + CONSUMER_WARPS * STG_WARP * 4 + 1024;
 constexpr int THREADS = 32 * CONSUMER_WARPS + 128; // + the producer warpgroup (one thread issues the TMA loads)
 // registers per thread after setmaxnreg: the launch gives every thread 65536 / 384 = 168; the producer warpgroup returns
-// what the consumers need for 2 x (64 + 32) live accumulator and drain floats (128 x 40 + 256 x 232 <= 65536)
+// what the consumers need for 128 live accumulator and 64 drain floats (128 x 40 + 256 x 232 <= 65536)
 constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
 static_assert(SLAB_BYTES % 1024 == 0, "slab stages must stay 1024-byte aligned");
 static_assert(SMEM_BYTES <= 227 * 1024, "shared memory budget");
@@ -516,10 +604,10 @@ __global__ void __launch_bounds__(slab::THREADS, 1) conv_tc32_slab_kernel(const 
     // read after wgmma_wait<0>: otherwise ptxas serializes every wgmma of the kernel (it then waits after each instruction).
     tc::setmaxnreg_inc<CONSUMER_REGS>();
     const int wg = warp >> 2;
-    constexpr uint32_t HI_A = tc::desc_hi_sw128(SLAB_X * 128);
-    constexpr uint32_t HI_B = tc::desc_hi_sw128(1024);
-    constexpr uint32_t BLK1 = 8 * 8;  // block 1 starts 8 slab positions (128 bytes = 8 descriptor units each) to the right
-    const uint32_t slab_lo0 = (tc::smem_u32(smem) >> 4) + static_cast<uint32_t>(8 * wg * SLAB_X * 8);
+    constexpr uint32_t HI_X = tc::desc_hi_sw128(SLAB_X * 128);   // B: groups of 8 positions one slab row apart
+    constexpr uint32_t HI_W = tc::desc_hi_sw128(1024);           // A: groups of 8 weight rows
+    // x-half wg starts 8 slab positions (128 bytes = 8 descriptor units each) to the right
+    const uint32_t slab_lo0 = (tc::smem_u32(smem) >> 4) + static_cast<uint32_t>(wg * 8 * 8);
     const uint32_t bt_lo0 = tc::smem_u32(smem_b) >> 4;
     int sa = 0; uint32_t pha = 0;
     int sb = 0; uint32_t phb = 0;
@@ -529,11 +617,11 @@ __global__ void __launch_bounds__(slab::THREADS, 1) conv_tc32_slab_kernel(const 
       const int y0 = (r / P.tiles_x) * TYP, x0 = (r % P.tiles_x) * TXP;
       // the tile's first group overwrites the accumulators (scale-d = 0); defining them here ends their live range at the
       // last drain, so that they hold no registers during the epilogue
-      float acc0[64], acc1[64], v0[32], v1[32];
+      float acc[128], v[64];
 #pragma unroll
-      for (int i = 0; i < 64; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; }
+      for (int i = 0; i < 128; ++i) acc[i] = 0.f;
 #pragma unroll
-      for (int i = 0; i < 32; ++i) { v0[i] = 0.f; v1[i] = 0.f; }
+      for (int i = 0; i < 64; ++i) v[i] = 0.f;
       int in_win = 0;  // channel blocks accumulated in the current window
       int pend_b = -1;
       for (int j = 0; j < nblk; ++j) {
@@ -550,24 +638,19 @@ __global__ void __launch_bounds__(slab::THREADS, 1) conv_tc32_slab_kernel(const 
           for (int par = 0; par < 2; ++par) {
             const int tap = 2 * tp + par;
             if (tap < 9) {   // odd tap: +64 bytes inside the weight row
-              const uint32_t a_t = slab_lo + static_cast<uint32_t>((tap / 3) * SLAB_X + (tap % 3)) * 8;
-              mma_block64<F>(acc0, a_t, HI_A, b_lo + par * 4, HI_B, tap == 0 ? fresh : 1u);
-              mma_block64<F>(acc1, a_t + BLK1, HI_A, b_lo + par * 4, HI_B, tap == 0 ? fresh : 1u);
+              const uint32_t x_t = slab_lo + static_cast<uint32_t>((tap / 3) * SLAB_X + (tap % 3)) * 8;
+              mma_block128<F>(acc, b_lo + par * 4, HI_W, x_t, HI_X, tap == 0 ? fresh : 1u);
             }
           }
           tc::wgmma_commit();
           if (tp == 4) {
             tc::wgmma_wait<0>();
-            tc::reg_fence<64>(acc0);
-            tc::reg_fence<64>(acc1);
+            tc::reg_fence<128>(acc);
             if (pend_b >= 0) release_stage(&bempty[pend_b]);
             release_stage(&bempty[sb]);
             release_stage(&aempty[sa]);
             pend_b = -1;
-            if (last_of_win) {
-              drain<F>(v0, acc0);
-              drain<F>(v1, acc1);
-            }
+            if (last_of_win) drain<F, 128>(v, acc);
           } else {
             tc::wgmma_wait<1>();
             if (pend_b >= 0) release_stage(&bempty[pend_b]);
@@ -578,16 +661,11 @@ __global__ void __launch_bounds__(slab::THREADS, 1) conv_tc32_slab_kernel(const 
         if (++sa == A_STAGES) { sa = 0; pha ^= 1; }
         in_win = last_of_win ? 0 : in_win + 1;
       }
-      float* stg = reinterpret_cast<float*>(smem_b + B_STAGES * WT_TILE) + warp * STG_WARP;
-#pragma unroll
-      for (int blk = 0; blk < 2; ++blk) {   // m64 block blk: x-half blk of the warpgroup's y-half
-        const auto pixel_of = [&](int m) -> long long {
-          const int mm = 16 * (warp & 3) + m;
-          const int y = y0 + 8 * wg + (mm >> 3), x = x0 + 8 * blk + (mm & 7);
-          return y < P.H && x < P.W ? ((long long)b * P.H + y) * P.W + x : -1;
-        };
-        epilogue<F>(P, blk ? v1 : v0, stg, pixel_of, nt * 64);
-      }
+      const auto pixel_of = [&](int n) -> long long {   // column n: slab row n / 8 of the warpgroup's x-half
+        const int y = y0 + (n >> 3), x = x0 + 8 * wg + (n & 7);
+        return y < P.H && x < P.W ? ((long long)b * P.H + y) * P.W + x : -1;
+      };
+      epilogue_t<F>(P, v, reinterpret_cast<float*>(smem_b + B_STAGES * WT_TILE) + warp * STG_WARP, pixel_of, nt * 64 + 16 * (warp & 3));
     }
   }
 }
@@ -1167,11 +1245,12 @@ static int conv_slab(const void* x, const void* weight, const float* bias, const
   static const int def_win = getenv("DINVK_TC32_SLAB_WINDOW") ? std::max(1, atoi(getenv("DINVK_TC32_SLAB_WINDOW"))) : 1;
   P.win = window > 0 ? window : def_win;
   P.tiles_x = ceil_div(W, slab::TXP); P.tiles_y = ceil_div(H, slab::TYP);
-  // N tiles of a pixel tile are adjacent work items in groups of at most 2, so that CTAs sharing a slab run together while
-  // only one weight group at a time is streamed (DINVK_TC32_NT_GROUP overrides: 1 = N tile outermost)
+  // N tiles of a pixel tile are adjacent work items in pairs, so that the two CTAs sharing a slab run together (the second
+  // reads it from L2: the 256- and 512-channel layers read their activations from HBM twice instead of 4 or 8 times) while
+  // only two weight groups at a time are streamed (DINVK_TC32_NT_GROUP overrides: 1 = N tile outermost)
   {
     static const int env_g = getenv("DINVK_TC32_NT_GROUP") ? atoi(getenv("DINVK_TC32_NT_GROUP")) : 0;
-    int g = env_g > 0 ? env_g : (P.n_tiles <= 2 ? P.n_tiles : 1);
+    int g = env_g > 0 ? env_g : 2;
     while (g > 1 && P.n_tiles % g) --g;
     P.ngrp = std::max(1, std::min(g, P.n_tiles));
   }
