@@ -340,6 +340,178 @@ __global__ void __launch_bounds__(256) svblur_adj_kernel(const __grid_constant__
   store_tile(out + (long long)bc * P.Hout * P.Wout, tot, P, i0, j0, tx, ty);
 }
 
+// ---- tiled space-varying blur (tiled product convolution) -------------------------------------------------------------------
+// A x = sum_k Wt_k . (h_k *valid x), A^T y = sum_k h_k (transposed valid) (Wt_k . y).  Patch k = r * nc + c covers rows
+// [r s1, r s1 + P1) and columns [c s2, c s2 + P2) of the compatible grid, whose origin is x's; its multiplier w_k (P1 x P2, shared
+// over B and C) is placed there, and Wt_k is that plane cropped to the valid output, which sits at (a_i, a_j) = (h/2, w/2).
+// A tile visits only the (r, c) rectangle of patches that can reach it, never all K.  Tile t of the grid has origin G = 64 t in
+// stage_patch's coordinates and stores outputs G - d.. (d_i, d_j below, rows and columns before 0 are masked): the forward uses
+// d = a, so its tiles lie on multiples of 64 of the compatible grid (one stride cell per tile when the stride is a multiple of 64
+// that divides the patch); the adjoint uses d = 32, which centres the tile's read span (64 + h - 1) on a multiple of 64.
+struct TsvParams {
+  BlurParams P;        // one term's geometry; Hout x Wout is the output plane
+  int K, nr, nc, P1, P2, s1, s2;
+  int ai, aj;          // compatible coordinates of y's origin
+  int di, dj;          // output origin of tile G = G - d
+  int Hy, Wy;          // y plane (the valid output)
+  int xs;              // adjoint: 1 = the y patch is staged once in shared memory, 0 = y is re-read through L1 / L2 for every term
+};
+
+// patches [*lo, *hi] along one dimension whose span [n s, n s + p) meets the compatible interval [a, b]; empty when *lo > *hi
+__device__ __forceinline__ void term_range(int a, int b, int p, int s, int n, int* lo, int* hi) {
+  const int e = a - p + 1;  // span end must pass a
+  *lo = e <= 0 ? 0 : (e + s - 1) / s;
+  *hi = a > b ? -1 : min(n - 1, b / s);  // (a >= 0 here)
+}
+
+__device__ __forceinline__ void store_tile_masked(float* __restrict__ dst, const float (&acc)[4][4], const BlurParams& P, int i0,
+                                                  int j0, int tx, int ty) {
+#pragma unroll
+  for (int r = 0; r < 4; ++r) {
+    const int gi = i0 + ty * 4 + r;
+    if (gi < 0 || gi >= P.Hout) continue;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const int gj = j0 + tx * 4 + q;
+      if (gj >= 0 && gj < P.Wout) dst[(long long)gi * P.Wout + gj] = acc[r][q];
+    }
+  }
+}
+
+// Forward.  The x patch is staged once; per term the correlation with the flipped h_k goes into a partial block, which is added
+// times w_k at every output pixel inside patch k (and nowhere else: a non-finite h_k reaches exactly its footprint).  A warp (8
+// output rows) skips the window loop of a term whose rows it does not meet.
+__global__ void __launch_bounds__(256) tiled_svblur_fwd_kernel(const __grid_constant__ tt::TileMap tmap, int use_tma,
+                                                               const float* __restrict__ x, const float* __restrict__ mult,
+                                                               const float* __restrict__ filt, float* __restrict__ y, TsvParams S) {
+  const BlurParams& P = S.P;
+  DINVK_DYN_SMEM(float, smem);
+  float* ks = smem;
+  float* patch = align128(smem + P.h * P.wp);
+  const int tid = threadIdx.x;
+  const int bc = blockIdx.y;
+  const int b = bc / P.C, c = bc - b * P.C;
+  const int gi = (blockIdx.x / P.tiles_x) * BL_T, gj = (blockIdx.x % P.tiles_x) * BL_T;
+  const int oi = gi - S.di, oj = gj - S.dj;  // output origin; compatible coordinates of the tile's outputs: o + a
+  int r0, r1, c0, c1;
+  term_range(max(oi, 0) + S.ai, min(oi + BL_T, P.Hout) - 1 + S.ai, S.P1, S.s1, S.nr, &r0, &r1);
+  term_range(max(oj, 0) + S.aj, min(oj + BL_T, P.Wout) - 1 + S.aj, S.P2, S.s2, S.nc, &c0, &c1);
+  if (r0 > r1 || c0 > c1) return;  // (uniform) a tile of masked outputs only
+  const float* fb = filt + ((long long)(P.FB == 1 ? 0 : b) * P.FC + (P.FC == 1 ? 0 : c)) * S.K * P.h * P.w;
+  stage_patch(patch, &tmap, use_tma, x + (long long)bc * P.Hin * P.Win, P, gi, gj, bc);
+
+  const int tx = tid & 15, ty = tid >> 4;
+  const int wr = oi + S.ai + (ty & ~1) * 4;  // first compatible row of this warp's outputs
+  float tot[4][4];
+#pragma unroll
+  for (int r = 0; r < 4; ++r)
+#pragma unroll
+    for (int q = 0; q < 4; ++q) tot[r][q] = 0.f;
+  for (int pr = r0; pr <= r1; ++pr) {
+    for (int pc = c0; pc <= c1; ++pc) {
+      const int k = pr * S.nc + pc;
+      __syncthreads();  // the window loop of the previous term is done with ks
+      stage_filter(ks, fb + (long long)k * P.h * P.w, P);
+      __syncthreads();  // (first term: the x patch has landed as well)
+      const int ri = oi + S.ai - pr * S.s1, rj = oj + S.aj - pc * S.s2;  // tile origin in patch k's multiplier plane
+      if (wr + 8 <= pr * S.s1 || wr >= pr * S.s1 + S.P1) continue;  // (warp-uniform)
+      float part[4][4];
+#pragma unroll
+      for (int r = 0; r < 4; ++r)
+#pragma unroll
+        for (int q = 0; q < 4; ++q) part[r][q] = 0.f;
+      window_fma(patch, ks, P, tx, ty, part);
+      const float* wk = mult + (long long)k * S.P1 * S.P2;
+#pragma unroll
+      for (int r = 0; r < 4; ++r) {
+        const int I = ri + ty * 4 + r;
+        if (I < 0 || I >= S.P1) continue;
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const int J = rj + tx * 4 + q;
+          if (J >= 0 && J < S.P2) tot[r][q] = fmaf(part[r][q], __ldg(wk + (long long)I * S.P2 + J), tot[r][q]);
+        }
+      }
+    }
+  }
+  store_tile_masked(y + (long long)bc * P.Hout * P.Wout, tot, P, oi, oj, tx, ty);
+}
+
+// Adjoint.  Per term: stage the unflipped h_k and the product patch Wt_k . y (zero outside patch k and outside y), run the window
+// loop into a partial block and add it at the output pixels within patch k's footprint grown by the filter (where a non-finite
+// h_k reaches in the reference, and the only pixels a finite one can change).  A warp skips terms whose grown rows it does not meet.
+__global__ void __launch_bounds__(256, 2) tiled_svblur_adj_kernel(const __grid_constant__ tt::TileMap tmap, int use_tma,
+                                                                  const float* __restrict__ yin, const float* __restrict__ mult,
+                                                                  const float* __restrict__ filt, float* __restrict__ out,
+                                                                  TsvParams S) {
+  const BlurParams& P = S.P;
+  DINVK_DYN_SMEM(float, smem);
+  const int PH = BL_T + P.h - 1;
+  float* ks = smem;
+  float* prod = align128(smem + P.h * P.wp);
+  float* yp = align128(prod + PH * P.PW);
+  const int tid = threadIdx.x;
+  const int bc = blockIdx.y;
+  const int b = bc / P.C, c = bc - b * P.C;
+  const int gi = (blockIdx.x / P.tiles_x) * BL_T, gj = (blockIdx.x % P.tiles_x) * BL_T;
+  const int oi = gi - S.di, oj = gj - S.dj;  // output origin (x coordinates = compatible coordinates)
+  // output rows [lo, hi] read y rows [lo - (h - 1), hi] (cut to y), i.e. compatible rows + a
+  int r0, r1, c0, c1;
+  term_range(max(max(oi, 0) - (P.h - 1), 0) + S.ai, min(min(oi + BL_T, P.Hout) - 1, S.Hy - 1) + S.ai, S.P1, S.s1, S.nr, &r0, &r1);
+  term_range(max(max(oj, 0) - (P.w - 1), 0) + S.aj, min(min(oj + BL_T, P.Wout) - 1, S.Wy - 1) + S.aj, S.P2, S.s2, S.nc, &c0, &c1);
+  if (r0 > r1 || c0 > c1) return;  // (uniform) a tile of masked outputs only
+  const float* fb = filt + ((long long)(P.FB == 1 ? 0 : b) * P.FC + (P.FC == 1 ? 0 : c)) * S.K * P.h * P.w;
+  const float* src = yin + (long long)bc * P.Hin * P.Win;
+  if (S.xs) stage_patch(yp, &tmap, use_tma, src, P, gi, gj, bc);
+
+  const int tx = tid & 15, ty = tid >> 4;
+  const int wr = oi + (ty & ~1) * 4;  // first output row of this warp
+  float tot[4][4];
+#pragma unroll
+  for (int r = 0; r < 4; ++r)
+#pragma unroll
+    for (int q = 0; q < 4; ++q) tot[r][q] = 0.f;
+  for (int pr = r0; pr <= r1; ++pr) {
+    for (int pc = c0; pc <= c1; ++pc) {
+      const int k = pr * S.nc + pc;
+      __syncthreads();  // the window loop of the previous term is done with ks and prod (first term: the y patch has landed)
+      stage_filter(ks, fb + (long long)k * P.h * P.w, P);
+      const float* wk = mult + (long long)k * S.P1 * S.P2;
+      const int pi = pr * S.s1 - S.ai, pj = pc * S.s2 - S.aj;  // patch k's origin in y coordinates
+      for (int idx = tid; idx < PH * P.PW; idx += 256) {
+        const int er = idx / P.PW, ec = idx - er * P.PW;
+        const int yi = gi + er + P.off_i, yj = gj + ec + P.off_j;
+        const int I = yi - pi, J = yj - pj;
+        float v = 0.f;
+        if (yi >= 0 && yi < S.Hy && yj >= 0 && yj < S.Wy && I >= 0 && I < S.P1 && J >= 0 && J < S.P2)
+          v = (S.xs ? yp[idx] : __ldg(src + (long long)yi * P.Win + yj)) * __ldg(wk + (long long)I * S.P2 + J);
+        prod[idx] = v;
+      }
+      __syncthreads();
+      // output rows patch k can reach: [pi, pi + P1 - 1 + h - 1] (y rows [pi, pi + P1) spread by the filter)
+      const int ei = pi + S.P1 + P.h - 1, ej = pj + S.P2 + P.w - 1;
+      if (wr + 8 <= pi || wr >= ei) continue;  // (warp-uniform)
+      float part[4][4];
+#pragma unroll
+      for (int r = 0; r < 4; ++r)
+#pragma unroll
+        for (int q = 0; q < 4; ++q) part[r][q] = 0.f;
+      window_fma(prod, ks, P, tx, ty, part);
+#pragma unroll
+      for (int r = 0; r < 4; ++r) {
+        const int i = oi + ty * 4 + r;
+        if (i < pi || i >= ei) continue;
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const int j = oj + tx * 4 + q;
+          if (j >= pj && j < ej) tot[r][q] += part[r][q];
+        }
+      }
+    }
+  }
+  store_tile_masked(out + (long long)bc * P.Hout * P.Wout, tot, P, oi, oj, tx, ty);
+}
+
 // transpose of replicate / reflect padding: x[p,q] = sum over the extended indices that the padding maps onto (p,q)
 // z is the extended image (He = H + h - 1 rows starting at extended index a_min = h/2 - h + 1; same for columns)
 __device__ __forceinline__ int preimages(int p, int n, int amin, int amax, int mode, int* start, int* count) {
@@ -468,6 +640,45 @@ static int run_svblur_adj(const float* y, const float* mult, const float* filt, 
   return DINVK_POST_LAUNCH();
 }
 
+// number of patches along one dimension of an n-pixel image padded at the end to the compatible size (utils/_tiling.py:27-46);
+// 0 when the image pads to less than one patch
+static long long tiled_count(long long n, long long p, long long s) {
+  const long long np = (n > p ? n - p : p - n) / s + 1;
+  const long long nc = n + (p + np * s - n) % s;
+  return nc >= p ? (nc - p) / s + 1 : 0;
+}
+
+// fwd: x (H x W) -> y (Ho x Wo), tiles on multiples of 64 of the compatible grid; adj: y -> x (H x W), tiles centred (d = 32).
+// The tile grid covers the output plus the d masked rows / columns before it.
+static int run_tiled_svblur(bool fwd, const float* in, const float* mult, const float* filt, float* out, int B, int C, int H, int W,
+                            int FB, int FC, int K, int nr, int nc, int h, int w, int P1, int P2, int s1, int s2, void* stream) {
+  const int Ho = H - h + 1, Wo = W - w + 1;
+  TsvParams S;
+  S.K = K; S.nr = nr; S.nc = nc; S.P1 = P1; S.P2 = P2; S.s1 = s1; S.s2 = s2;
+  S.ai = h / 2; S.aj = w / 2; S.Hy = Ho; S.Wy = Wo;
+  S.di = fwd ? S.ai : BL_T / 2; S.dj = fwd ? S.aj : BL_T / 2;
+  S.P = fwd ? corr_params(C, H, W, Ho, Wo, FB, FC, h, w, 1, -S.di, -S.dj, 0)
+            : corr_params(C, Ho, Wo, H, W, FB, FC, h, w, 0, -(h - 1) - S.di, -(w - 1) - S.dj, 0);
+  S.P.tiles_x = ceil_div(S.P.Wout + S.dj, BL_T);
+  const size_t one = filter_bytes(S.P) + patch_bytes(S.P) + 128, two = one + patch_bytes(S.P) + 128;
+  if (one > BL_SMEM_BUDGET) return set_error(DINVK_EUNSUPPORTED, "tiled_svblur: filter %dx%d too large for the tiled kernel", h, w);
+  S.xs = !fwd && two <= BL_SMEM_BUDGET;
+  const size_t smem = S.xs ? two : one;
+  int rc = fwd ? allow_smem(tiled_svblur_fwd_kernel, smem) : allow_smem(tiled_svblur_adj_kernel, smem);
+  if (rc) return rc;
+  BlurParams G = S.P;  // the grid: tile_grid counts ceil(Hout / 64) rows of tiles; this grid has d more rows
+  G.Hout += S.di;
+  dim3 grid;
+  tt::TileMap tmap;
+  int use_tma;
+  if ((rc = tile_grid(G, B, C, in, fwd || S.xs, &grid, &tmap, &use_tma))) return rc;
+  if (fwd)
+    DINVK_LAUNCH(tiled_svblur_fwd_kernel, grid, dim3(256), smem, stream, tmap, use_tma, in, mult, filt, out, S);
+  else
+    DINVK_LAUNCH(tiled_svblur_adj_kernel, grid, dim3(256), smem, stream, tmap, use_tma, in, mult, filt, out, S);
+  return DINVK_POST_LAUNCH();
+}
+
 static int check_blur_args(const void* a, const void* f, const void* o, int B, int C, int H, int W, int FB, int FC, int h, int w,
                            int padding) {
   DINVK_CHECK_ARG(a && f && o, "blur: null pointer");
@@ -568,4 +779,29 @@ extern "C" int dinvk_svblur_adj(const float* y, const float* mult, const float* 
     return rc;
   DINVK_LAUNCH(blur_fold_kernel, dim3(ceil_div((long long)H * W, 256), B * C), dim3(256), 0, stream, (const float*)z, x, H, W, h, w, mode);
   return DINVK_POST_LAUNCH();
+}
+
+// ---- tiled space-varying blur: deepinv/physics/blur.py:871-1192 (TiledSpaceVaryingBlur.A / A_adjoint) and
+// deepinv/physics/functional/tiled_product_convolution.py (the multipliers); valid padding only ------------------------------
+static int tiled_svblur(bool fwd, const float* in, const float* mult, const float* filt, float* out, int B, int C, int H, int W,
+                        int FB, int FC, int K, int h, int w, int P1, int P2, int s1, int s2, void* stream) {
+  DINVK_CHECK_ARG(mult, "tiled_svblur: null multipliers");
+  DINVK_CHECK_ARG(P1 >= 1 && P2 >= 1 && s1 >= 1 && s2 >= 1, "tiled_svblur: bad patch (%d,%d) / stride (%d,%d)", P1, P2, s1, s2);
+  DINVK_CHECK_ARG(s1 <= P1 && s2 <= P2, "tiled_svblur: stride (%d,%d) larger than the patch (%d,%d)", s1, s2, P1, P2);
+  int rc = check_blur_args(in, filt, out, B, C, H, W, FB, FC, h, w, DINVK_PAD_VALID);
+  if (rc) return rc;
+  const long long nr = tiled_count(H, P1, s1), nc = tiled_count(W, P2, s2);
+  DINVK_CHECK_ARG(nr >= 1 && nc >= 1 && nr * nc == K, "tiled_svblur: %lld x %lld patches on a %dx%d image, %d filters", nr, nc, H, W, K);
+  if (B == 0) return DINVK_OK;
+  return run_tiled_svblur(fwd, in, mult, filt, out, B, C, H, W, FB, FC, K, (int)nr, (int)nc, h, w, P1, P2, s1, s2, stream);
+}
+
+extern "C" int dinvk_tiled_svblur_fwd(const float* x, const float* mult, const float* filt, float* y, int B, int C, int H, int W,
+                                      int FB, int FC, int K, int h, int w, int P1, int P2, int s1, int s2, void* stream) {
+  return tiled_svblur(true, x, mult, filt, y, B, C, H, W, FB, FC, K, h, w, P1, P2, s1, s2, stream);
+}
+
+extern "C" int dinvk_tiled_svblur_adj(const float* y, const float* mult, const float* filt, float* x, int B, int C, int H, int W,
+                                      int FB, int FC, int K, int h, int w, int P1, int P2, int s1, int s2, void* stream) {
+  return tiled_svblur(false, y, mult, filt, x, B, C, H, W, FB, FC, K, h, w, P1, P2, s1, s2, stream);
 }

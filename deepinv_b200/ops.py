@@ -457,6 +457,42 @@ def svblur_adj(y, mult, filt, padding: int, H: int, W: int) -> torch.Tensor:
     return x
 
 
+def _tiled_svblur_shapes(mult, filt):
+    _, _, K, P1, P2 = mult.shape
+    FB, FC, Kf, h, w = filt.shape
+    if Kf != K:
+        raise ValueError(f"tiled_svblur: {K} multipliers for {Kf} filters")
+    return FB, FC, K, h, w, P1, P2
+
+
+def tiled_svblur_fwd(x, mult, filt, stride) -> torch.Tensor:
+    """y = sum_k Wt_k . (filt[:, :, k] *valid x): x (B,C,H,W), mult (1,1,K,P1,P2), filt (FB,FC,K,h,w), stride (s1, s2)"""
+    dev = _require_cuda(x, mult, filt)
+    x, mult, filt = _f32c(x), _f32c(mult), _f32c(filt)
+    B, C, H, W = x.shape
+    FB, FC, K, h, w, P1, P2 = _tiled_svblur_shapes(mult, filt)
+    y = torch.empty(B, C, H - h + 1, W - w + 1, dtype=torch.float32, device=dev)
+    if y.numel() == 0:
+        return y
+    check(get_lib().dinvk_tiled_svblur_fwd(_p(x), _p(mult), _p(filt), _p(y), B, C, H, W, FB, FC, K, h, w, P1, P2, *stride,
+                                           _stream(dev)))
+    return y
+
+
+def tiled_svblur_adj(y, mult, filt, stride, H: int, W: int) -> torch.Tensor:
+    """the transpose of tiled_svblur_fwd onto a (B,C,H,W) image"""
+    dev = _require_cuda(y, mult, filt)
+    y, mult, filt = _f32c(y), _f32c(mult), _f32c(filt)
+    B, C = y.shape[:2]
+    FB, FC, K, h, w, P1, P2 = _tiled_svblur_shapes(mult, filt)
+    x = torch.empty(B, C, H, W, dtype=torch.float32, device=dev)
+    if x.numel() == 0:
+        return x
+    check(get_lib().dinvk_tiled_svblur_adj(_p(y), _p(mult), _p(filt), _p(x), B, C, H, W, FB, FC, K, h, w, P1, P2, *stride,
+                                           _stream(dev)))
+    return x
+
+
 # --------------------------------------------------------------------------------------------
 # denoiser convolutions, bf16 tensor-core path (NHWC bf16 activations)
 # --------------------------------------------------------------------------------------------

@@ -1,5 +1,5 @@
 from . import functional, generator  # noqa: F401
-from .blur import Blur, BlurFFT, Downsampling, SpaceVaryingBlur  # noqa: F401
+from .blur import Blur, BlurFFT, Downsampling, SpaceVaryingBlur, TiledSpaceVaryingBlur  # noqa: F401
 from .forward import DecomposablePhysics, LinearPhysics, Physics  # noqa: F401
 from .mri import MRI, DynamicMRI, MRIMixin, MultiCoilMRI, SequentialMRI, TimeMixin  # noqa: F401
 from .noise import GaussianNoise, NoiseModel, ZeroNoise  # noqa: F401

@@ -8,7 +8,8 @@ and its rfft2-domain U/V methods, but A / A_adjoint / A_adjoint_A / prox_l2 / A_
 fused launches of `dinvk_spectral` on PAIRS of real images packed as one complex image (a real
 filter commutes with the packing), so a (B,C,H,W) batch costs B*C/2 complex 2-D transforms.
 `SpaceVaryingBlur` (blur.py:740-868) is the product convolution sum_k h_k * (w_k . x) on one fused kernel per direction
-(`dinvk_svblur_fwd / _adj`, csrc/blur.cu).
+(`dinvk_svblur_fwd / _adj`, csrc/blur.cu), and `TiledSpaceVaryingBlur` (blur.py:871-1192) its tiled form with one PSF per
+overlapping patch (`dinvk_tiled_svblur_fwd / _adj`).
 """
 from __future__ import annotations
 
@@ -118,6 +119,103 @@ class SpaceVaryingBlur(LinearPhysics):
         if padding is not None:
             self.padding = padding
         super().update_parameters(filters=filters, multipliers=multipliers, **kwargs)
+
+
+class TiledSpaceVaryingBlur(LinearPhysics):
+    r"""y = sum_k Wt_k . (h_k * x), space-varying blur by tiled product convolution (blur.py:871-1192): one PSF per
+    overlapping patch, blended by a partition of unity, valid padding.
+
+    :param torch.Tensor filters: h_k, (b, c, K, h, w) with b in {1, B}, c in {1, C}; K = nr * nc patches, row-major.
+    :param int, tuple[int, int] patch_size: patch (P1, P2).
+    :param int, tuple[int, int] stride: stride (s1, s2) <= patch; defaults to half the patch.
+    :param str blending_mode: 'bump' or 'linear' (`functional.generate_tiled_multipliers`).
+    :param bool use_fft: stored as in the reference, where it selects FFT convolutions: the same operator up to rounding.
+        Both values run the direct fused kernel here.
+
+    The image is padded at the bottom / right to the compatible size that nr x nc patches tile; a patch reaching into that
+    padding still counts where it overlaps the image.  `A` and `A_adjoint` take ``filters=`` and store them; the multipliers
+    (buffer `multipliers`, (1, 1, K, P1, P2)) are regenerated only when the image size changes.  One fused kernel per direction
+    (`dinvk_tiled_svblur_fwd / _adj`); gradients flow to x only.  `A_dagger`, `prox_l2` and the norm estimate are the CG /
+    power-method versions of LinearPhysics."""
+
+    def __init__(self, filters: Tensor = None, patch_size=None, stride=None, blending_mode: str = "bump", use_fft: bool = True,
+                 device="cpu", dtype=torch.float32, **kwargs):
+        from .functional import _resolve_tiling_params
+
+        super().__init__(device=device, **kwargs)
+        self.patch_size, self.stride = _resolve_tiling_params(patch_size, stride)
+        self.pad_if_needed = True
+        self.blending_mode = blending_mode
+        self.use_fft = use_fft
+        self._dynamic_img_size = None
+        self.register_buffer("filters", filters)
+        self.register_buffer("multipliers", None)
+        self.to(device=device, dtype=dtype)
+
+    @staticmethod
+    def num_filters(img_size, patch_size, stride=None) -> tuple[int, int]:
+        """patches (nr, nc) along each dimension, hence the number of filters nr * nc, for an image of `img_size`"""
+        from .functional import _as_pair, _num_patches, _resolve_tiling_params
+
+        return _num_patches(_as_pair(img_size), *_resolve_tiling_params(patch_size, stride))
+
+    def get_num_patches(self, img_size) -> tuple[int, int]:
+        from .functional import _as_pair, _num_patches
+
+        return _num_patches(_as_pair(img_size), self.patch_size, self.stride)
+
+    def get_needed_pad(self, img_size) -> tuple[int, int]:
+        from .functional import _as_pair, _needed_pad
+
+        return _needed_pad(_as_pair(img_size), self.patch_size, self.stride)
+
+    def get_compatible_img_size(self, img_size) -> tuple[int, int]:
+        from .functional import _as_pair, _compatible_size
+
+        return _compatible_size(_as_pair(img_size), self.patch_size, self.stride)
+
+    def _operands(self, t: Tensor, H: int, W: int):
+        """the reference's failure modes on an (H, W) image"""
+        h, w = self.filters, self.multipliers
+        nr, nc = self.get_num_patches((H, W))
+        if nr * nc != h.size(2):
+            raise ValueError(f"The total number of patches must be equal to the number of PSFs, got {nr * nc} and {h.size(2)}")
+        if tuple(w.shape) != (1, 1, nr * nc, *self.patch_size):
+            raise NotImplementedError(f"multipliers of shape {tuple(w.shape)}: only the shared (1, 1, K, P1, P2) blending of "
+                                      "generate_tiled_multipliers is supported")
+        if t.dim() != 4:
+            raise ValueError(f"Input image must have shape (B, C, H, W), got {tuple(t.shape)}.")
+        _check_filter(h, t.size(0), t.size(1))
+        return w, h
+
+    def A(self, x: Tensor, filters: Tensor = None, **kwargs) -> Tensor:
+        H, W = x.shape[-2:]
+        self.update_parameters(filters, img_size=(H, W), device=x.device, **kwargs)
+        w, h = self._operands(x, H, W)
+        return linear_apply(x, lambda t: ops.tiled_svblur_fwd(t, w, h, self.stride),
+                            lambda t: ops.tiled_svblur_adj(t, w, h, self.stride, H, W))
+
+    def A_adjoint(self, y: Tensor, filters: Tensor = None, **kwargs) -> Tensor:
+        # valid padding: the image is the measurement grown by the filter
+        fh, fw = (self.filters if filters is None else filters).shape[-2:]
+        H, W = y.shape[-2] + fh - 1, y.shape[-1] + fw - 1
+        self.update_parameters(filters, img_size=(H, W), device=y.device, **kwargs)
+        w, h = self._operands(y, H, W)
+        return linear_apply(y, lambda t: ops.tiled_svblur_adj(t, w, h, self.stride, H, W),
+                            lambda t: ops.tiled_svblur_fwd(t, w, h, self.stride))
+
+    def update_parameters(self, filters: Tensor = None, img_size=None, device=None, **kwargs):
+        from .functional import generate_tiled_multipliers
+
+        if isinstance(filters, Tensor):
+            self.register_buffer("filters", filters.to(device) if device is not None else filters)
+        if img_size is not None and (self.multipliers is None or tuple(img_size) != self._dynamic_img_size
+                                     or (device is not None and self.multipliers.device != torch.device(device))):
+            w = generate_tiled_multipliers(self.get_compatible_img_size(img_size), self.patch_size, self.stride,
+                                           mode=self.blending_mode, device=device if device is not None else "cpu")
+            self.register_buffer("multipliers", w)
+            self._dynamic_img_size = tuple(img_size)
+        super().update_parameters(**kwargs)
 
 
 class BlurFFT(DecomposablePhysics):

@@ -1,11 +1,12 @@
-"""Filter constructors used by Blur / BlurFFT / Downsampling (deepinv/physics/functional/blur.py:137-372,552-583), and the
-product convolution of SpaceVaryingBlur (deepinv/physics/functional/product_convolution.py:10-68).
+"""Filter constructors used by Blur / BlurFFT / Downsampling (deepinv/physics/functional/blur.py:137-372,552-583), the
+product convolution of SpaceVaryingBlur (deepinv/physics/functional/product_convolution.py:10-68), and the patch geometry and
+blending multipliers of TiledSpaceVaryingBlur (deepinv/utils/_tiling.py:12-61, functional/tiled_product_convolution.py).
 
 Filter generation is host-side (a few hundred taps): plain torch on whatever device is asked for; the operators that
 consume these filters, and the product convolution itself, run on the libdinvk kernels."""
 from __future__ import annotations
 
-from math import pi, sqrt
+from math import exp, pi, sqrt
 
 import torch
 
@@ -141,3 +142,76 @@ def product_convolution2d_adjoint(y: torch.Tensor, w: torch.Tensor, h: torch.Ten
     H, W = (y.shape[-2] + fh - 1, y.shape[-1] + fw - 1) if padding.lower() == "valid" else tuple(y.shape[-2:])
     w, h, code = _product_convolution_args(y, w, h, padding, H, W)
     return linear_apply(y, lambda t: ops.svblur_adj(t, w, h, code, H, W), lambda t: ops.svblur_fwd(t, w, h, code))
+
+
+# ---- tiled space-varying blur: patch geometry (deepinv/utils/_tiling.py:12-61) and multipliers --------------------------------
+def _as_pair(v) -> tuple[int, int]:
+    return (v, v) if isinstance(v, int) else tuple(v)
+
+
+def _resolve_tiling_params(patch_size, stride=None) -> tuple[tuple[int, int], tuple[int, int]]:
+    patch_size = _as_pair(patch_size)
+    stride = _as_pair(stride) if stride is not None else tuple(p // 2 for p in patch_size)
+    if stride[0] > patch_size[0] or stride[1] > patch_size[1]:
+        raise ValueError(f"Stride {stride} must be smaller or equal than patch_size {patch_size}.")
+    return patch_size, stride
+
+
+def _needed_pad(img_size, patch_size, stride) -> tuple[int, int]:
+    """rows / columns of zeros added at the bottom / right so that the patches tile the image"""
+    return tuple((p + (abs(n - p) // s + 1) * s - n) % s for n, p, s in zip(img_size, patch_size, stride))
+
+
+def _compatible_size(img_size, patch_size, stride) -> tuple[int, int]:
+    return tuple(n + d for n, d in zip(img_size, _needed_pad(img_size, patch_size, stride)))
+
+
+def _num_patches(img_size, patch_size, stride) -> tuple[int, int]:
+    return tuple((n - p) // s + 1 for n, p, s in zip(_compatible_size(img_size, patch_size, stride), patch_size, stride))
+
+
+def bump_function(x: torch.Tensor, a: float = 1.0, b: float = 1.0) -> torch.Tensor:
+    """1 on [-a, a], a smooth bump down to 0 on [-a-b, -a] and [a, a+b] (deepinv/physics/generator/blur.py:1014-1047)"""
+    abs_x = torch.abs(x)
+    t = (abs_x - a) / b
+    safe_t = t.clamp(0.0, 1.0 - 1e-6)
+    transition = torch.exp(-1.0 / (1.0 - safe_t ** 2)) / exp(-1.0)
+    return torch.where(abs_x <= a, 1.0, torch.where(abs_x < a + b, transition, 0.0))
+
+
+def _unity_partition_1d(n: int, patch: int, stride: int, mode: str, dtype) -> torch.Tensor:
+    """(n_patch, n) masks summing to 1 along each column (tiled_product_convolution.py:9-59)"""
+    n_patch = (n - patch) // stride + 1
+    max_size = patch + (n_patch - 1) * stride
+    overlap = patch - stride
+    t = torch.linspace(-max_size // 2, max_size // 2, max_size, dtype=dtype)
+    if mode.lower() == "bump":
+        mask = bump_function(t, patch / 2 - overlap, overlap).roll(shifts=-max_size // 2 + patch // 2)
+    elif mode.lower() == "linear":
+        a, b = patch / 2 - overlap, overlap
+        mask = ((a + b) / b - t.abs().clip(0, a + b) / b).abs().clip(0, 1)  # b = 0 (stride == patch): ZeroDivisionError
+        mask = mask.roll(shifts=-max_size // 2 + patch // 2)
+    else:
+        raise ValueError(f"Unknown mode: {mode}. Use 'bump' or 'linear'.")
+    masks = torch.stack([mask.roll(shifts=stride * i) for i in range(n_patch)], dim=0)
+    masks[0, :stride] = 1.0
+    masks[-1, -stride:] = 1.0
+    return masks / (masks.sum(dim=0, keepdims=True) + 1e-8)
+
+
+def generate_tiled_multipliers(img_size, patch_size, stride, mode: str = "bump", device="cpu",
+                               dtype=torch.float32) -> torch.Tensor:
+    r"""The blending multipliers of TiledSpaceVaryingBlur, (1, 1, K, P1, P2) (tiled_product_convolution.py:105-143): the outer
+    product of two 1-D partitions of unity, renormalised over the K patches, cut to each patch.  Host-side parameter
+    generation: evaluated on the CPU in `dtype` with the reference's operations (so float32 gives the reference's CPU values bit
+    for bit), then copied to `device` once.  The normaliser is the reference's sum over the (nr, nc, H, W) product, which takes
+    4 K H W bytes of host memory for a moment."""
+    img_size, patch_size, stride = _as_pair(img_size), _as_pair(patch_size), _as_pair(stride)
+    mx = _unity_partition_1d(img_size[0], patch_size[0], stride[0], mode, dtype)
+    my = _unity_partition_1d(img_size[1], patch_size[1], stride[1], mode, dtype)
+    masks = torch.tensordot(mx, my, dims=0).permute(0, 2, 1, 3)
+    norm = masks.sum(dim=(0, 1)) + 1e-8
+    (P1, P2), (s1, s2) = patch_size, stride
+    w = torch.stack([masks[i, j, i * s1: i * s1 + P1, j * s2: j * s2 + P2] / norm[i * s1: i * s1 + P1, j * s2: j * s2 + P2]
+                     for i in range(mx.size(0)) for j in range(my.size(0))])
+    return w[None, None].to(device)

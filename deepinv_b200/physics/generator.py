@@ -208,3 +208,28 @@ class MotionBlurGenerator(PSFGenerator):
         kernel = hist.reshape(batch_size, 1, h, w)
         kernel = kernel / (kernel.sum(dim=(-2, -1), keepdim=True) + 1e-6)
         return {"filter": kernel}
+
+
+class TiledBlurGenerator(PSFGenerator):
+    r"""Filters of TiledSpaceVaryingBlur (generator/blur.py:1737-1799): one PSF of `psf_generator` per patch of the image.
+    `step(batch_size, img_size, seed)` draws batch_size * K PSFs in one call of `psf_generator` and returns
+    ``{"filters": (B, C, K, h, w)}`` with the reference's reshape, so a CPU generator with the same seed gives its filters."""
+
+    def __init__(self, psf_generator: PSFGenerator, patch_size, stride=None, rng: torch.Generator | None = None, device="cpu",
+                 **kwargs):
+        from .functional import _resolve_tiling_params
+
+        super().__init__(psf_size=psf_generator.psf_size, rng=rng, device=device, **kwargs)
+        self.patch_size, self.stride = _resolve_tiling_params(patch_size, stride)
+        self.pad_if_needed = True
+        self.psf_generator = psf_generator
+
+    def get_num_patches(self, img_size) -> tuple[int, int]:
+        from .functional import _as_pair, _num_patches
+
+        return _num_patches(_as_pair(img_size), self.patch_size, self.stride)
+
+    def step(self, batch_size: int = 1, img_size=None, seed: int | None = None, **kwargs) -> dict:
+        nr, nc = self.get_num_patches(img_size)
+        psf = self.psf_generator.step(batch_size=batch_size * nr * nc, seed=seed, **kwargs)["filter"]
+        return {"filters": psf.view(batch_size, nr * nc, -1, *self.psf_size).transpose(1, 2)}

@@ -230,6 +230,19 @@ int dinvk_svblur_adj(const float* y, const float* mult, const float* filt, float
                      int MB, int MC, int FB, int FC, int K, int h, int w, int padding,
                      void* workspace, size_t workspace_bytes, void* stream);
 
+/* Tiled space-varying blur (deepinv/physics/blur.py:871-1192, TiledSpaceVaryingBlur.A / A_adjoint; multipliers from
+ * deepinv/physics/functional/tiled_product_convolution.py:105-143), valid padding:
+ *   y = sum_k Wt_k . (h_k * x),  x = sum_k h_k^T * (Wt_k . y).
+ * x (B,C,H,W) in both directions, y (B,C,H-h+1,W-w+1), filters (FB,FC,K,h,w) with FB in {1,B}, FC in {1,C}, multipliers
+ * (K,P1,P2) shared over B and C.  The image is padded at the bottom / right to the compatible size of patch (P1,P2) and
+ * stride (s1,s2) (deepinv/utils/_tiling.py:27-46), which holds nr x nc patches; patch k = r*nc + c covers rows
+ * [r*s1, r*s1+P1) and columns [c*s2, c*s2+P2), and Wt_k is its multiplier placed there and cropped to y, which starts at
+ * (h/2, w/2).  DINVK_EINVAL unless nr*nc == K and 1 <= s <= P.  One launch, no workspace, no atomics. */
+int dinvk_tiled_svblur_fwd(const float* x, const float* mult, const float* filt, float* y, int B, int C, int H, int W,
+                           int FB, int FC, int K, int h, int w, int P1, int P2, int s1, int s2, void* stream);
+int dinvk_tiled_svblur_adj(const float* y, const float* mult, const float* filt, float* x, int B, int C, int H, int W,
+                           int FB, int FC, int K, int h, int w, int P1, int P2, int s1, int s2, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Denoiser convolutions (deepinv/models/drunet.py:200-210,323-433; dncnn.py:116-131)
  * ------------------------------------------------------------------------------------------
