@@ -114,7 +114,9 @@ __global__ void __launch_bounds__(128) radon_fwd_kernel(const float* __restrict_
   float acc = 0.f;
   const Trig45 tq = trig45(cos_t, sin_t, G.A, t);
   long long PX, PY;
-  sample_pos45(tq, G.P, j, i0, PX, PY);
+  // (a ray that misses the support has i0 > i1 and possibly i0 far beyond P: its start position is never used, but is kept in
+  // range so the Q45 products cannot overflow)
+  sample_pos45(tq, G.P, j, min(i0, G.P - 1), PX, PY);
   for (int i = i0; i <= i1; ++i, PX += tq.s, PY += tq.c) {
     int X0, Y0;
     float wx0, wx1, wy0, wy1;
@@ -245,7 +247,50 @@ constexpr int RTW = 76;   // staged row pitch / box width (floats): columns ox-3
                           // this round, started the box at ox = 64 tx - 1 and trapped as an illegal instruction)
 constexpr int RXO = 3;    // index of column ox inside a staged row
 constexpr int RTH = 66;   // staged rows
+// transpose: columns 69 .. 75 of each accumulator row are never added to (the owned floors end at offset 64, their right taps at
+// 65 = column 68); columns RNF .. RNF+4 hold 2 bits per owned floor cell of the row (65 cells) that mark NaN / Inf samples
+constexpr int RNF = 70;
 constexpr int RT_THREADS = 128;
+
+// steps i of ray j whose sample can fall in the tile [fxl, fxu) x [fyl, fyu) (padded coordinates), +- 2 steps of margin for the
+// fp32 estimate: fxl <= bx + s (i - cx) < fxu and fyl <= by + c (i - cx) < fyu
+__device__ __forceinline__ void tile_steps(float c, float s, int j, float cx, float pm1, int P, float fxl, float fxu, float fyl,
+                                           float fyu, int& i0, int& i1) {
+  float i_lo = 0.f, i_hi = pm1;
+  const float bx = cx + c * ((float)j - cx), by = cx - s * ((float)j - cx);
+  if (fabsf(s) > 1e-6f) {
+    float a = (fxl - bx) / s + cx, b = (fxu - bx) / s + cx;
+    if (a > b) { const float tmp = a; a = b; b = tmp; }
+    i_lo = fmaxf(i_lo, a); i_hi = fminf(i_hi, b);
+  } else if (!(bx > fxl - 1.f && bx < fxu + 1.f)) { i_hi = -1.f; }
+  if (fabsf(c) > 1e-6f) {
+    float a = (fyl - by) / c + cx, b = (fyu - by) / c + cx;
+    if (a > b) { const float tmp = a; a = b; b = tmp; }
+    i_lo = fmaxf(i_lo, a); i_hi = fminf(i_hi, b);
+  } else if (!(by > fyl - 1.f && by < fyu + 1.f)) { i_hi = -1.f; }
+  i0 = max(0, (int)floorf(i_lo) - 2);
+  i1 = min(P - 1, (int)ceilf(i_hi) + 2);
+}
+
+// rays j of angle (c, s) that can reach the tile [fxl, fxu) x [fyl, fyu): j ~ cx + c (X - cx) - s (Y - cx) over its corners, +- 1
+__device__ __forceinline__ void tile_rays(float c, float s, float cx, int P, float fxl, float fxu, float fyl, float fyu, int& jmin,
+                                          int& jmax) {
+  const float j00 = c * (fxl - cx) - s * (fyl - cx), j10 = c * (fxu - cx) - s * (fyl - cx);
+  const float j01 = c * (fxl - cx) - s * (fyu - cx), j11 = c * (fxu - cx) - s * (fyu - cx);
+  jmin = max(0, (int)floorf(cx + fminf(fminf(j00, j10), fminf(j01, j11))) - 1);
+  jmax = min(P - 1, (int)ceilf(cx + fmaxf(fmaxf(j00, j10), fmaxf(j01, j11))) + 1);
+}
+
+// non-finite samples of the transpose, by floor cell (ux, uy) of the tile: 1 = +Inf, 2 = -Inf, 3 = NaN, ORed (+Inf and -Inf
+// together give NaN, as in an fp32 sum)
+__device__ __forceinline__ void mark_nonfinite(int* TI, int ux, int uy, float v) {
+  const int code = (v != v) ? 3 : (v > 0.f ? 1 : 2);
+  atomicOr(TI + uy * RTW + RNF + (ux >> 4), code << (2 * (ux & 15)));
+}
+__device__ __forceinline__ int nonfinite_mark(const int* TI, int ux, int uy) {
+  if (ux < 0 || uy < 0 || ux > RT || uy > RT) return 0;
+  return (TI[uy * RTW + RNF + (ux >> 4)] >> (2 * (ux & 15))) & 3;
+}
 
 template <bool ADJ>
 __global__ void __launch_bounds__(RT_THREADS) radon_tiled_kernel(const __grid_constant__ tt::TileMap tmap, int use_tma,
@@ -267,7 +312,7 @@ __global__ void __launch_bounds__(RT_THREADS) radon_tiled_kernel(const __grid_co
   float* T = reinterpret_cast<float*>(rt_al);
   int* TI = reinterpret_cast<int*>(rt_al);
   long long* s_cs = reinterpret_cast<long long*>(rt_al + (((size_t)RTH * RTW * 4 + 15) & ~(size_t)15));  // cos[A], sin[A], Q45
-  __shared__ unsigned s_absmax;
+  __shared__ unsigned s_absmax[2];  // transpose: max |y| over the tile's rays, max over the finite ones
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int ty = blockIdx.x / tps, tx = blockIdx.x - ty * tps;
   const int bc = blockIdx.y;
@@ -297,7 +342,7 @@ __global__ void __launch_bounds__(RT_THREADS) radon_tiled_kernel(const __grid_co
     }
   } else {
     for (int e = tid; e < RTH * RTW; e += RT_THREADS) TI[e] = 0;
-    if (tid == 0) s_absmax = 0u;
+    if (tid == 0) { s_absmax[0] = 0u; s_absmax[1] = 0u; }
   }
   for (int k = tid; k < G.A; k += RT_THREADS) { const Trig45 q = trig45(cos_t, sin_t, G.A, k); s_cs[k] = q.c; s_cs[G.A + k] = q.s; }
   __syncthreads();
@@ -319,63 +364,82 @@ __global__ void __launch_bounds__(RT_THREADS) radon_tiled_kernel(const __grid_co
   float fx_scale = 1.f;
   double fx_inv = 1.0;
   if (ADJ) {
-    // fixed-point scale of this tile: sf = 0.999 * 2^30 / (2 A m), m = max |y| over the rays that can reach the tile (the
-    // bits of a non-negative float order like unsigned integers).  At one angle the bilinear weights of the lattice samples
-    // around a pixel sum to 1 +- 0.1 (a tent function summed over a rotated unit lattice), bounded here by 2: a pixel
-    // collects at most 2 A m, i.e. < 2^30 after scaling — no overflow.  One unit is 2 A m / 2^30 (A = 180: 3.4e-7 m); the
-    // rounding errors of a pixel's ~4 A contributions add up like a random walk to ~8 units: 2.6e-6 m, i.e. 1e-6 .. 2e-6 of the
-    // pixel value for white-noise and for ramp-filtered sinograms — an order of magnitude below the fp32 coordinate noise of
-    // the reference's own transpose at this size, and independent of the order of the adds.
-    unsigned m = 0u;
-    for (int t = warp; t < G.A; t += RT_THREADS / 32) {
-      const float c = (float)s_cs[t] * 2.842170943040401e-14f, s = (float)s_cs[G.A + t] * 2.842170943040401e-14f;
-      const float j00 = c * (fxl - cx) - s * (fyl - cx), j10 = c * (fxu - cx) - s * (fyl - cx);
-      const float j01 = c * (fxl - cx) - s * (fyu - cx), j11 = c * (fxu - cx) - s * (fyu - cx);
-      const int jmin = max(0, (int)floorf(cx + fminf(fminf(j00, j10), fminf(j01, j11))) - 1);
-      const int jmax = min(G.P - 1, (int)ceilf(cx + fmaxf(fmaxf(j00, j10), fmaxf(j01, j11))) + 1);
-      for (int j = jmin + lane; j <= jmax; j += 32) m = max(m, __float_as_uint(fabsf(__ldg(src + srow0 + (long long)t * G.P + j) * scale)));
-    }
+    // fixed-point scale of this tile: sf = 0.999 * 2^30 / (2 A m), m = max |y| over the finite values of the rays that can
+    // reach the tile (the bits of a non-negative float order like unsigned integers; NaN and Inf order above every finite
+    // value and are left out: the pixels they reach are marked and overwritten, see below).  At one angle the bilinear weights of the lattice
+    // samples around a pixel sum to between 0.83 and 1 + 4 (1 - 1/sqrt(2))^2 = 1.343 (a tent function summed over a rotated
+    // unit lattice; the maximum is at 45 degrees on a lattice point, tests/test_radon_ref64.py), bounded here by 2: a pixel
+    // collects at most 1.343 A m < 2 A m, i.e. < 2^30 after scaling — no overflow.  One unit is 2 A m / 2^30 (A = 180:
+    // 3.4e-7 m); the rounding errors of a pixel's ~4 A contributions add up like a random walk to ~8 units: 2.6e-6 m, i.e.
+    // 1e-6 .. 2e-6 of the pixel value for white-noise and for ramp-filtered sinograms — an order of magnitude below the fp32
+    // coordinate noise of the reference's own transpose at this size, and independent of the order of the adds.
+    // (NaN and Inf order above every finite value: when the first sweep meets one, a second takes the largest finite |y|)
+    for (int pass = 0; pass < 2; ++pass) {
+      unsigned m = 0u;
+      for (int t = warp; t < G.A; t += RT_THREADS / 32) {
+        const float c = (float)s_cs[t] * 2.842170943040401e-14f, s = (float)s_cs[G.A + t] * 2.842170943040401e-14f;
+        int jmin, jmax;
+        tile_rays(c, s, cx, G.P, fxl, fxu, fyl, fyu, jmin, jmax);
+        for (int j = jmin + lane; j <= jmax; j += 32) {
+          const unsigned b = __float_as_uint(fabsf(__ldg(src + srow0 + (long long)t * G.P + j) * scale));
+          m = max(m, (pass == 0 || b < 0x7f800000u) ? b : 0u);
+        }
+      }
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
-    if (lane == 0) atomicMax(&s_absmax, m);
-    __syncthreads();
-    const float mf = __uint_as_float(s_absmax);
-    if (mf > 0.f && mf < 3.0e38f) {
+      for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
+      if (lane == 0) atomicMax(&s_absmax[pass], m);
+      __syncthreads();
+      if (s_absmax[0] < 0x7f800000u) break;
+    }
+    const float mf = __uint_as_float(s_absmax[s_absmax[0] < 0x7f800000u ? 0 : 1]);
+    if (mf > 0.f) {
       fx_scale = (0.999f * 1073741824.0f / (float)(2 * G.A)) / mf;
       if (!(fx_scale < 3.0e38f)) fx_scale = 3.0e38f;   // denormal-sized sinograms
     }
     fx_inv = 1.0 / (double)fx_scale;
   }
+  if (ADJ && s_absmax[0] >= 0x7f800000u) {
+    // a NaN / Inf ray cannot go through the integer accumulator (NaN would convert to 0, Inf saturate and wrap): this pass
+    // marks the floor cells of its samples in the tile (RNF); the final add turns the four taps of a marked cell into that
+    // non-finite value, whatever the main loop's integer adds left there.  Marks only, in shared memory, and before the main loop: so placed, the kernel keeps the 48 registers
+    // it has without this pass (fp32 atomics to the image from a pass after the main loop took 60).
+    for (int t = warp; t < G.A; t += RT_THREADS / 32) {
+      Trig45 tq;
+      tq.c = s_cs[t]; tq.s = s_cs[G.A + t];
+      const float c = (float)tq.c * 2.842170943040401e-14f, s = (float)tq.s * 2.842170943040401e-14f;
+      int jmin, jmax;
+      tile_rays(c, s, cx, G.P, fxl, fxu, fyl, fyu, jmin, jmax);
+      for (int j = jmin + lane; j <= jmax; j += 32) {
+        const float yv = __ldg(src + srow0 + (long long)t * G.P + j) * scale;
+        if (fabsf(yv) <= 3.402823466e38f) continue;
+        int i0, i1;
+        tile_steps(c, s, j, cx, pm1, G.P, fxl, fxu, fyl, fyu, i0, i1);
+        long long PX, PY;
+        sample_pos45(tq, G.P, j, min(i0, G.P - 1), PX, PY);
+        for (int i = i0; i <= i1; ++i, PX += tq.s, PY += tq.c) {
+          const unsigned ux = (unsigned)((int)(PX >> 45) - xl), uy = (unsigned)((int)(PY >> 45) - yl);
+          if (ux > (unsigned)xr || uy > (unsigned)yr) continue;
+          mark_nonfinite(TI, ux, uy, yv);
+        }
+      }
+    }
+  }
   for (int t = warp; t < G.A; t += RT_THREADS / 32) {
     Trig45 tq;
     tq.c = s_cs[t]; tq.s = s_cs[G.A + t];
     const float c = (float)tq.c * 2.842170943040401e-14f, s = (float)tq.s * 2.842170943040401e-14f;
-    // ray range of the tile: j ~ cx + c (X - cx) - s (Y - cx) over the corners of [xl, xu+1] x [yl, yu+1]
-    const float j00 = c * (fxl - cx) - s * (fyl - cx), j10 = c * (fxu - cx) - s * (fyl - cx);
-    const float j01 = c * (fxl - cx) - s * (fyu - cx), j11 = c * (fxu - cx) - s * (fyu - cx);
-    const int jmin = max(0, (int)floorf(cx + fminf(fminf(j00, j10), fminf(j01, j11))) - 1);
-    const int jmax = min(G.P - 1, (int)ceilf(cx + fmaxf(fmaxf(j00, j10), fmaxf(j01, j11))) + 1);
+    int jmin, jmax;
+    tile_rays(c, s, cx, G.P, fxl, fxu, fyl, fyu, jmin, jmax);
     for (int j = jmin + lane; j <= jmax; j += 32) {
-      // steps whose sample can fall in the tile: fxl <= bx + s (i - cx) < fxu and fyl <= by + c (i - cx) < fyu (+- 2 margin)
-      float i_lo = 0.f, i_hi = pm1;
-      const float bx = cx + c * ((float)j - cx), by = cx - s * ((float)j - cx);
-      if (fabsf(s) > 1e-6f) {
-        float a = (fxl - bx) / s + cx, b = (fxu - bx) / s + cx;
-        if (a > b) { const float tmp = a; a = b; b = tmp; }
-        i_lo = fmaxf(i_lo, a); i_hi = fminf(i_hi, b);
-      } else if (!(bx > fxl - 1.f && bx < fxu + 1.f)) { i_hi = -1.f; }
-      if (fabsf(c) > 1e-6f) {
-        float a = (fyl - by) / c + cx, b = (fyu - by) / c + cx;
-        if (a > b) { const float tmp = a; a = b; b = tmp; }
-        i_lo = fmaxf(i_lo, a); i_hi = fminf(i_hi, b);
-      } else if (!(by > fyl - 1.f && by < fyu + 1.f)) { i_hi = -1.f; }
-      const int i0 = max(0, (int)floorf(i_lo) - 2), i1 = min(G.P - 1, (int)ceilf(i_hi) + 2);
+      int i0, i1;
+      tile_steps(c, s, j, cx, pm1, G.P, fxl, fxu, fyl, fyu, i0, i1);
       float acc = 0.f;
       float yv = 0.f;
       if (ADJ && i0 <= i1) yv = (__ldg(src + srow0 + (long long)t * G.P + j) * scale) * fx_scale;
+      // (a NaN / Inf ray's integer adds land only on the taps of the cells the pass above marked, which the final add overwrites)
       bool any = false;
       long long PX, PY;
-      sample_pos45(tq, G.P, j, i0, PX, PY);
+      sample_pos45(tq, G.P, j, min(i0, G.P - 1), PX, PY);  // i0 > i1 (not used) may lie far beyond P, see radon_fwd_kernel
       for (int i = i0; i <= i1; ++i, PX += tq.s, PY += tq.c) {
         int X0, Y0;
         float wx0, wx1, wy0, wy1;
@@ -406,6 +470,11 @@ __global__ void __launch_bounds__(RT_THREADS) radon_tiled_kernel(const __grid_co
       const int x = ox + ux, y = oy + uy;
       if (x < 0 || x >= G.W || y < 0 || y >= G.W) continue;
       float v = (float)((double)TI[uy * RTW + ux + RXO] * fx_inv);
+      if (s_absmax[0] >= 0x7f800000u) {  // the taps (ux, uy) of the cells (ux - 1 .. ux, uy - 1 .. uy)
+        const int code = nonfinite_mark(TI, ux, uy) | nonfinite_mark(TI, ux - 1, uy) | nonfinite_mark(TI, ux, uy - 1) |
+                         nonfinite_mark(TI, ux - 1, uy - 1);
+        if (code) v = __uint_as_float(code == 1 ? 0x7f800000u : (code == 2 ? 0xff800000u : 0x7fc00000u));
+      }
       if (G.circle) {
         const float ax = 2.0f * (float)x / (float)(G.W - 1) - 1.0f, ay = 2.0f * (float)y / (float)(G.W - 1) - 1.0f;
         if (!(ax * ax + ay * ay <= 1.0f)) v = 0.f;
@@ -545,8 +614,10 @@ extern "C" int dinvk_radon_adj(const float* sino, float* x, int BC, int W, int P
     rc = launch_tiled(true, nullptr, sino, x, BC, G, cos_t, sin_t, scale, stream);
     if (rc >= 0) return rc;
   }
-  DINVK_LAUNCH(radon_adj_kernel, dim3(ceil_div((long long)W * W, 256), BC), dim3(256), 2 * A * sizeof(long long), stream, sino, x, G,
-               cos_t, sin_t, scale);
+  // the Q45 tables: 2 A * 8 bytes, above the default 48 KB for A > 3072
+  const size_t smem = 2 * (size_t)A * sizeof(long long);
+  if ((rc = allow_smem(radon_adj_kernel, smem))) return rc;
+  DINVK_LAUNCH(radon_adj_kernel, dim3(ceil_div((long long)W * W, 256), BC), dim3(256), smem, stream, sino, x, G, cos_t, sin_t, scale);
   return DINVK_POST_LAUNCH();
 }
 
@@ -558,8 +629,9 @@ extern "C" int dinvk_iradon_bp(const float* sino, float* x, int BC, int W, int P
   if (rc) return rc;
   if (BC == 0) return DINVK_OK;
   DINVK_CHECK_ARG(BC <= 65535 && A <= 4096, "dinvk_iradon_bp: grid too large");
-  DINVK_LAUNCH(iradon_bp_kernel, dim3(ceil_div((long long)W * W, 256), BC), dim3(256), 2 * A * sizeof(float), stream, sino, x, G,
-               cos_t, sin_t, scale);
+  const size_t smem = 2 * (size_t)A * sizeof(float);
+  if ((rc = allow_smem(iradon_bp_kernel, smem))) return rc;
+  DINVK_LAUNCH(iradon_bp_kernel, dim3(ceil_div((long long)W * W, 256), BC), dim3(256), smem, stream, sino, x, G, cos_t, sin_t, scale);
   return DINVK_POST_LAUNCH();
 }
 
