@@ -16,7 +16,7 @@
 //     A^T replicate/reflect  : no flip, off = -(h-1), zeros -> extended (H+h-1, W+w-1) image, then the
 //                              transpose of the padding folds the border strips back (fold kernel).
 // A CTA computes a 64x64 output tile; each thread owns 4x4 outputs and slides a 4-wide register window
-// along the filter row (one 128-bit shared load per 16 FMAs per row).  Filters up to ~128x128 fit.
+// along the filter row (one 128-bit shared load per 16 FMAs per row).  Filters up to 123x123 fit (200 KB of shared memory).
 //
 // The space-varying blur (product convolution, SpaceVaryingBlur) runs the same tile and window loop K times per CTA, once per
 // term, into one set of accumulators: svblur_fwd_kernel on the product patch w_k . x, svblur_adj_kernel on the y patch with a
@@ -215,6 +215,29 @@ __global__ void __launch_bounds__(256) blur_corr_kernel(const __grid_constant__ 
         lo[r] = hi;
       }
     }
+  }
+  // The window loop also runs the zero taps (the `shift` leading ones and the pad to wp) against real patch values, and 0 * NaN =
+  // 0 * Inf = NaN: a non-finite pixel would reach up to 8 columns instead of its w-column footprint.  Such a zero tap adds 0 *
+  // finite = +-0 to every other output, so only a non-finite accumulator can carry the leak; it is recomputed from the real taps
+  // v in [shift, shift + w), in the loop's u-major order (the patch and filter stay resident: no barrier).  One rolled loop over
+  // the flagged outputs: a repair unrolled per output took 66 registers, this form 48 (sm_90a), 0 spills.
+  unsigned bad = 0;
+#pragma unroll
+  for (int r = 0; r < 4; ++r)
+#pragma unroll
+    for (int q = 0; q < 4; ++q) bad |= (unsigned)((__float_as_uint(acc[r][q]) & 0x7f800000u) == 0x7f800000u) << (4 * r + q);
+#pragma unroll 1
+  for (int e = 0; bad >> e; ++e) {
+    if (!((bad >> e) & 1)) continue;
+    const float* prow = &patch[(ty * 4 + (e >> 2)) * P.PW + tx * 4 + (e & 3)];
+    float a = 0.f;
+    for (int u = 0; u < P.h; ++u)
+      for (int v = P.shift; v < P.shift + P.w; ++v) a = fmaf(ks[u * P.wp + v], prow[u * P.PW + v], a);
+#pragma unroll
+    for (int r = 0; r < 4; ++r)
+#pragma unroll
+      for (int q = 0; q < 4; ++q)
+        if (4 * r + q == e) acc[r][q] = a;
   }
   float* dst = out + (long long)bc * P.Hout * P.Wout;
 #pragma unroll
@@ -550,12 +573,13 @@ __global__ void __launch_bounds__(256) blur_fold_kernel(const float* __restrict_
 }
 
 static BlurParams corr_params(int C, int Hin, int Win, int Hout, int Wout, int FB, int FC, int h, int w, int flip, int off_i, int off_j,
-                              int map) {
+                              int map, bool align = true) {
   BlurParams P;
   // A tensor-map box has to start on a 16-byte boundary of the image row.  Tiles start at multiples of 64 columns, so the patch
   // origin j0 + off_j is aligned iff off_j is a multiple of 4: prepend shift = off_j mod 4 zero taps to the filter rows and move
   // the origin left by as much (out[j] = sum_v ks'[v] in[j + v + off_j - shift], ks'[v] = ks[v - shift]): same sums, aligned box.
-  const int shift = ((off_j % 4) + 4) % 4;
+  // align = false keeps the unshifted layout (mapped-loop staging only).
+  const int shift = align ? ((off_j % 4) + 4) % 4 : 0;
   off_j -= shift;
   P.shift = shift;
   P.C = C; P.Hin = Hin; P.Win = Win; P.Hout = Hout; P.Wout = Wout; P.h = h; P.w = w; P.wp = (w + shift + 3) & ~3;
@@ -588,15 +612,24 @@ static int tile_grid(const BlurParams& P, int B, int C, const float* in, bool wa
 
 static int run_corr(const float* in, const float* filt, float* out, int B, int C, int Hin, int Win, int Hout, int Wout,
                     int FB, int FC, int h, int w, int flip, int off_i, int off_j, int map, void* stream) {
-  const BlurParams P = corr_params(C, Hin, Win, Hout, Wout, FB, FC, h, w, flip, off_i, off_j, map);
-  const size_t smem = filter_bytes(P) + patch_bytes(P) + 128;
+  BlurParams P = corr_params(C, Hin, Win, Hout, Wout, FB, FC, h, w, flip, off_i, off_j, map);
+  size_t smem = filter_bytes(P) + patch_bytes(P) + 128;
+  // The shift taps widen the rows by up to 4 (to the next multiple of 4), and off_j differs between A and A^T: at the budget line
+  // the aligned layout of one direction can miss while the other fits.  The unshifted layout, staged by the mapped loop (its box
+  // would not be aligned), makes the accepted filters the same in both directions: up to 123 x 123, 1 x 720 and 613 x 1.
+  bool aligned = true;
+  if (smem > BL_SMEM_BUDGET && P.shift) {
+    P = corr_params(C, Hin, Win, Hout, Wout, FB, FC, h, w, flip, off_i, off_j, map, false);
+    smem = filter_bytes(P) + patch_bytes(P) + 128;
+    aligned = false;
+  }
   if (smem > BL_SMEM_BUDGET) return set_error(DINVK_EUNSUPPORTED, "blur: filter %dx%d too large for the tiled kernel", h, w);
   int rc = allow_smem(blur_corr_kernel, smem);
   if (rc) return rc;
   dim3 grid;
   tt::TileMap tmap;
   int use_tma;
-  if ((rc = tile_grid(P, B, C, in, true, &grid, &tmap, &use_tma))) return rc;
+  if ((rc = tile_grid(P, B, C, in, aligned, &grid, &tmap, &use_tma))) return rc;
   DINVK_LAUNCH(blur_corr_kernel, grid, dim3(256), smem, stream, tmap, use_tma, in, filt, out, P);
   return DINVK_POST_LAUNCH();
 }

@@ -91,17 +91,20 @@ with torch.no_grad():
         ys = p.A(xs)
         report("Tomography.prox_l2 (CG<=50) batch 4", t(lambda: p.prox_l2(xs, ys, 1.0), 1, 1, graph=False))
     if "blur" in which:
-        B, H, W, k = 32, 1024, 1024, 31
+        B, H, W = 32, 1024, 1024
         x = torch.rand(B, 1, H, W, device=dev, generator=g)
-        f = torch.rand(1, 1, k, k, device=dev, generator=g)
-        f /= f.sum()
         img = B * H * W * 4 / 1e6
-        gf = 2 * k * k * B * H * W / 1e9
-        for pad in ("circular", "valid", "reflect"):
-            p = dinv.physics.Blur(filter=f, padding=pad, device=dev)
-            y = p.A(x)
-            report(f"Blur.A 32x1024^2 31x31 [{pad}]", t(lambda: p.A(x), 5, 2), 2 * img, gflop=gf)
-            report(f"Blur.A_adjoint [{pad}]", t(lambda: p.A_adjoint(y), 5, 2), 2 * img, gflop=gf)
+        for k in (31, 3):  # 3 x 3: the fewest FMAs per output, where a per-tile fixed cost shows most
+            f = torch.rand(1, 1, k, k, device=dev, generator=g)
+            f /= f.sum()
+            gf = 2 * k * k * B * H * W / 1e9
+            for pad in ("circular", "valid", "reflect", "replicate", "constant"):
+                p = dinv.physics.Blur(filter=f, padding=pad, device=dev)
+                y = p.A(x)
+                report(f"Blur.A 32x1024^2 {k}x{k} [{pad}]", t(lambda: p.A(x), 20, 3), 2 * img, gflop=gf)
+                report(f"Blur.A_adjoint {k}x{k} [{pad}]", t(lambda: p.A_adjoint(y), 20, 3), 2 * img, gflop=gf)
+        f = torch.rand(1, 1, 31, 31, device=dev, generator=g)
+        f /= f.sum()
         pf = dinv.physics.BlurFFT(img_size=(1, H, W), filter=f, device=dev)
         y = pf.A(x)
         report("BlurFFT.A 32x1024^2", t(lambda: pf.A(x), 10, 2), 2 * img)
