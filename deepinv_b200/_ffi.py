@@ -54,6 +54,9 @@ _SIGNATURES = {
     "dinvk_blur_fwd": (c_int, [c_void_p, c_void_p, c_void_p] + [c_int] * 9 + [c_void_p]),
     "dinvk_blur_adj_workspace_bytes": (c_size_t, [c_int] * 7),
     "dinvk_blur_adj": (c_int, [c_void_p, c_void_p, c_void_p] + [c_int] * 9 + [c_void_p, c_size_t, c_void_p]),
+    "dinvk_blur3d_fwd": (c_int, [c_void_p, c_void_p, c_void_p] + [c_int] * 11 + [c_void_p]),
+    "dinvk_blur3d_adj_workspace_bytes": (c_size_t, [c_int] * 9),
+    "dinvk_blur3d_adj": (c_int, [c_void_p, c_void_p, c_void_p] + [c_int] * 11 + [c_void_p, c_size_t, c_void_p]),
     "dinvk_svblur_fwd": (c_int, [c_void_p] * 4 + [c_int] * 12 + [c_void_p]),
     "dinvk_svblur_adj_workspace_bytes": (c_size_t, [c_int] * 7),
     "dinvk_svblur_adj": (c_int, [c_void_p] * 4 + [c_int] * 12 + [c_void_p, c_size_t, c_void_p]),

@@ -723,6 +723,299 @@ static int check_blur_args(const void* a, const void* f, const void* o, int B, i
   return 0;
 }
 
+// ---- 3-D blur (volumetric direct convolution) -------------------------------------------------------------------------------
+// The correlation of the file header with a depth axis under the same rules:
+//     out[z,i,j] = sum_{t,u,v} ks[t,u,v] * in[map(z + t + off_z), map(i + u + off_i), map(j + v + off_j)]
+//     A,  same-size paddings : flip (all three axes), off_z = d/2 - (d-1),  map = padding rule,  out (D, H, W)
+//     A,  valid              : flip, off_z = 0,                             no map,              out (D-d+1, H-h+1, W-w+1)
+//     A^T valid              : no flip, off_z = -(d-1), zeros,             in (D-d+1, H-h+1, W-w+1), out (D, H, W)
+//     A^T circular/constant  : no flip, off_z = -d/2, circular/zeros                                out (D, H, W)
+//     A^T replicate/reflect  : no flip, off_z = -(d-1), zeros -> extended (D+d-1, H+h-1, W+w-1) volume, then the transpose of
+//                              the padding, a product of per-axis maps, folds it back (blur3d_fold_kernel, one gather)
+// A CTA owns a 64 x 64 tile of zt consecutive output planes of one (b, c) volume and walks the zt + d - 1 input planes that reach
+// them.  Each plane's tile + halo is staged once, by the TMA box or the mapped loop exactly as in 2-D (the depth index is mapped
+// before the box is issued: third coordinate b*C*D + map(z)); a plane outside the volume under zero padding is skipped.  The
+// staged plane p feeds every output plane k it reaches, with filter slice t = p - k, through the 2-D kernel's 4-wide register
+// window: each plane is read from global memory once and used up to zt times.  Filter slices stream through a ring of
+// zt + nbuf - 1 slots, one new slice per plane, so the depth of the filter is not limited.  With two patch buffers the next
+// plane's load (a TMA box in flight on its own mbarrier) runs under the current plane's FMAs.
+constexpr int B3_ZT = 4;  // output planes per CTA: 4 x 16 accumulators per thread
+
+struct Blur3dParams {
+  BlurParams P;     // one plane's geometry, as blur_corr_kernel runs it
+  int Din, Dout, d, off_z;
+  int zt, nbuf, ring;  // output planes per CTA (1 or B3_ZT), patch buffers (1 or 2), filter-slice slots (zt + nbuf - 1)
+  int ntiles;          // 64 x 64 tiles per plane; blockIdx.x = plane group * ntiles + tile
+};
+
+// depth t of the filter as the window loop reads it (flip reverses the depth axis; stage_filter reverses the other two)
+__device__ __forceinline__ void stage_slice3d(float* ks, const float* __restrict__ f, const Blur3dParams& S, int t) {
+  const BlurParams& P = S.P;
+  stage_filter(ks, f + (long long)(P.flip ? S.d - 1 - t : t) * P.h * P.w, P);
+}
+
+// The non-finite repair of blur_corr_kernel, in 3-D: the staged planes are gone by the end of the walk, so the one output is
+// recomputed from global memory over the real taps only (runs for non-finite accumulators alone).  Not inlined: inline, its
+// registers pushed the kernel past 128 and into spills in the window loop.
+#ifndef DINVK_EMUL
+__device__ __noinline__
+#endif
+float recompute3d(const float* __restrict__ src, const float* __restrict__ f, const Blur3dParams& S, int z, int i, int j) {
+  const BlurParams& P = S.P;
+  const long long pl = (long long)P.Hin * P.Win;
+  float a = 0.f;
+  for (int t = 0; t < S.d; ++t) {
+    bool okz;
+    const int gz = map_index(z + t + S.off_z, S.Din, P.map, okz);
+    if (!okz) continue;
+    const float* ft = f + (long long)(P.flip ? S.d - 1 - t : t) * P.h * P.w;
+    for (int u = 0; u < P.h; ++u) {
+      bool okr;
+      const int gi = map_index(i + u + P.off_i, P.Hin, P.map, okr);
+      if (!okr) continue;
+      for (int v = 0; v < P.w; ++v) {
+        bool okc;
+        const int gj = map_index(j + v + P.shift + P.off_j, P.Win, P.map, okc);
+        if (!okc) continue;
+        const float k = P.flip ? __ldg(ft + (P.h - 1 - u) * P.w + (P.w - 1 - v)) : __ldg(ft + u * P.w + v);
+        a = fmaf(k, __ldg(src + gz * pl + (long long)gi * P.Win + gj), a);
+      }
+    }
+  }
+  return a;
+}
+
+__global__ void __launch_bounds__(256, 2) blur3d_corr_kernel(const __grid_constant__ tt::TileMap tmap, int use_tma,
+                                                          const float* __restrict__ in, const float* __restrict__ filt,
+                                                          float* __restrict__ out, Blur3dParams S) {
+  const BlurParams& P = S.P;
+  DINVK_DYN_SMEM(float, smem);
+  const int PH = BL_T + P.h - 1, slice = P.h * P.wp;
+  float* ring = smem;                               // [ring][h][wp]
+  float* const buf0 = align128(smem + S.ring * slice);  // [PH][PW] patch buffers, 128-byte aligned (TMA destinations)
+  float* const buf1 = align128(buf0 + PH * P.PW);
+  const int tid = threadIdx.x;
+  const int bc = blockIdx.y;
+  const int b = bc / P.C, c = bc - b * P.C;
+  const int zg = blockIdx.x / S.ntiles, tile = blockIdx.x - zg * S.ntiles;
+  const int i0 = (tile / P.tiles_x) * BL_T, j0 = (tile % P.tiles_x) * BL_T;
+  const int z0 = zg * S.zt, nz = min(S.zt, S.Dout - z0), np = nz + S.d - 1;
+  const float* f = filt + ((long long)(P.FB == 1 ? 0 : b) * P.FC + (P.FC == 1 ? 0 : c)) * S.d * P.h * P.w;
+  const long long pl = (long long)P.Hin * P.Win;
+  const float* vol = in + (long long)bc * S.Din * pl;
+  bool by_tma = false;
+#ifndef DINVK_EMUL
+  __shared__ __align__(8) uint64_t bars[2];  // bars[p & 1]: the box of plane p
+  if (use_tma) {
+    const int r0 = i0 + P.off_i, c0 = j0 + P.off_j;
+    by_tma = (P.map == 0) || (r0 >= 0 && r0 + PH <= P.Hin && c0 >= 0 && c0 + P.PW <= P.Win);
+    if (by_tma && tid == 0) {  // (uniform over the CTA) published to the other threads by the plane loop's first barrier
+      tc::mbar_init(&bars[0], 1);
+      tc::mbar_init(&bars[1], 1);
+      tc::fence_barrier_init();
+    }
+  }
+  uint32_t phase = 0;  // bit n: parity of the next completion of bars[n]
+#else
+  (void)tmap; (void)use_tma;
+#endif
+  // plane p reads input depth map(z0 + p + off_z); false: outside the volume under zero padding (no staging, no FMAs)
+  auto depth = [&](int p, int* gz) {
+    bool ok;
+    *gz = map_index(z0 + p + S.off_z, S.Din, P.map, ok);
+    return ok;
+  };
+  // filter slice p into the ring and plane p's patch into buffer p % nbuf (no barrier: the caller's publishes)
+  auto stage = [&](int p) {
+    if (p < S.d) stage_slice3d(ring + (p % S.ring) * slice, f, S, p);
+    int gz;
+    if (!depth(p, &gz)) return;
+    float* patch = (p % S.nbuf) ? buf1 : buf0;
+#ifndef DINVK_EMUL
+    if (by_tma) {
+      if (tid == 0) {
+        tc::mbar_arrive_expect_tx(&bars[p & 1], (uint32_t)(PH * P.PW * 4));
+        tt::tma_load_3d(patch, &tmap, &bars[p & 1], j0 + P.off_j, i0 + P.off_i, bc * S.Din + gz);
+      }
+      return;
+    }
+#endif
+    const float* src = vol + gz * pl;
+    for (int idx = tid; idx < PH * P.PW; idx += 256) {
+      const int pr = idx / P.PW, pc = idx - pr * P.PW;
+      bool okr, okc;
+      const int gi = map_index(i0 + pr + P.off_i, P.Hin, P.map, okr);
+      const int gj = map_index(j0 + pc + P.off_j, P.Win, P.map, okc);
+      patch[idx] = (okr && okc) ? __ldg(src + (long long)gi * P.Win + gj) : 0.f;
+    }
+  };
+
+  const int tx = tid & 15, ty = tid >> 4;
+  float acc[B3_ZT][4][4];
+#pragma unroll
+  for (int k = 0; k < B3_ZT; ++k)
+#pragma unroll
+    for (int r = 0; r < 4; ++r)
+#pragma unroll
+      for (int q = 0; q < 4; ++q) acc[k][r][q] = 0.f;
+  if (S.nbuf == 2) stage(0);
+  for (int p = 0; p < np; ++p) {
+    // every thread is done with plane p - 1: its buffer and the ring slot of slice p + 1 - ring are free
+    __syncthreads();
+    if (S.nbuf == 2) {
+      if (p + 1 < np) stage(p + 1);
+    } else {
+      stage(p);
+      __syncthreads();
+    }
+    int gz;
+    if (!depth(p, &gz)) continue;  // (uniform)
+    const float* patch = (p % S.nbuf) ? buf1 : buf0;
+#ifndef DINVK_EMUL
+    if (by_tma) {
+      tc::mbar_wait(&bars[p & 1], (phase >> (p & 1)) & 1u);
+      phase ^= 1u << (p & 1);
+    }
+#endif
+    const int klo = max(0, p - S.d + 1), khi = min(nz - 1, p);  // output planes this plane reaches
+    if (klo == 0 && khi == B3_ZT - 1) {
+      // all B3_ZT planes: one pass of the window over the patch, each row chunk applied to the B3_ZT slices.  The sums of every
+      // accumulator run in window_fma's order, so this pass and the per-plane one below give the same bits.
+      const float* ks[B3_ZT];
+#pragma unroll
+      for (int k = 0; k < B3_ZT; ++k) ks[k] = ring + ((p - k) % S.ring) * slice;
+      const int nchunk = P.wp >> 2;
+      for (int u = 0; u < P.h; ++u) {
+        float4 lo[4];
+#pragma unroll
+        for (int r = 0; r < 4; ++r) lo[r] = *reinterpret_cast<const float4*>(&patch[(ty * 4 + r + u) * P.PW + tx * 4]);
+        for (int vb = 0; vb < nchunk; ++vb) {
+          float4 k4[B3_ZT];
+#pragma unroll
+          for (int k = 0; k < B3_ZT; ++k) k4[k] = reinterpret_cast<const float4*>(ks[k] + u * P.wp)[vb];
+#pragma unroll
+          for (int r = 0; r < 4; ++r) {
+            const float4 hi = *reinterpret_cast<const float4*>(&patch[(ty * 4 + r + u) * P.PW + tx * 4 + 4 * vb + 4]);
+            const float win[8] = {lo[r].x, lo[r].y, lo[r].z, lo[r].w, hi.x, hi.y, hi.z, hi.w};
+#pragma unroll
+            for (int k = 0; k < B3_ZT; ++k)
+#pragma unroll
+              for (int q = 0; q < 4; ++q) {
+                float a = acc[k][r][q];
+                a = fmaf(k4[k].x, win[q], a);
+                a = fmaf(k4[k].y, win[q + 1], a);
+                a = fmaf(k4[k].z, win[q + 2], a);
+                a = fmaf(k4[k].w, win[q + 3], a);
+                acc[k][r][q] = a;
+              }
+            lo[r] = hi;
+          }
+        }
+      }
+    } else {
+#pragma unroll
+      for (int k = 0; k < B3_ZT; ++k)
+        if (k >= klo && k <= khi) window_fma(patch, ring + ((p - k) % S.ring) * slice, P, tx, ty, acc[k]);
+    }
+  }
+  // The zero taps (shift and pad to wp) meet real patch values in the window loop, and 0 * NaN = NaN: as in blur_corr_kernel, a
+  // non-finite accumulator is recomputed over the real taps, so a NaN voxel reaches exactly its d x h x w footprint.
+#pragma unroll
+  for (int k = 0; k < B3_ZT; ++k) {
+    if (k >= nz) continue;
+    unsigned bad = 0;
+#pragma unroll
+    for (int r = 0; r < 4; ++r)
+#pragma unroll
+      for (int q = 0; q < 4; ++q) bad |= (unsigned)((__float_as_uint(acc[k][r][q]) & 0x7f800000u) == 0x7f800000u) << (4 * r + q);
+#pragma unroll 1
+    for (int e = 0; bad >> e; ++e) {
+      const int i = i0 + ty * 4 + (e >> 2), j = j0 + tx * 4 + (e & 3);
+      if (!((bad >> e) & 1) || i >= P.Hout || j >= P.Wout) continue;
+      const float a = recompute3d(vol, f, S, z0 + k, i, j);
+#pragma unroll
+      for (int r = 0; r < 4; ++r)
+#pragma unroll
+        for (int q = 0; q < 4; ++q)
+          if (4 * r + q == e) acc[k][r][q] = a;
+    }
+    store_tile(out + ((long long)bc * S.Dout + z0 + k) * P.Hout * P.Wout, acc[k], P, i0, j0, tx, ty);
+  }
+}
+
+// transpose of replicate / reflect padding in 3-D: x[s,p,q] = sum of the extended (D+d-1, H+h-1, W+w-1) volume over the product
+// of the per-axis preimages of s, p and q (blur_fold_kernel's rule on each axis)
+__global__ void __launch_bounds__(256) blur3d_fold_kernel(const float* __restrict__ z, float* __restrict__ x, int D, int H, int W,
+                                                          int d, int h, int w, int mode) {
+  const int bc = blockIdx.y;
+  const long long HW = (long long)H * W, idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= D * HW) return;
+  const int s = (int)(idx / HW), rem = (int)(idx - s * HW), p = rem / W, q = rem - p * W;
+  const int zmin = d / 2 - d + 1, amin = h / 2 - h + 1, bmin = w / 2 - w + 1;
+  const int De = D + d - 1, He = H + h - 1, We = W + w - 1;
+  int ds[3], dc[3], rs[3], rc[3], cs[3], cc[3];
+  const int nd = preimages(s, D, zmin, D - 1 + d / 2, mode, ds, dc);
+  const int nr = preimages(p, H, amin, H - 1 + h / 2, mode, rs, rc);
+  const int ncol = preimages(q, W, bmin, W - 1 + w / 2, mode, cs, cc);
+  const float* zz = z + (long long)bc * De * He * We;
+  float acc = 0.f;
+  for (int g = 0; g < nd; ++g)
+    for (int sa = ds[g]; sa < ds[g] + dc[g]; ++sa)
+      for (int a = 0; a < nr; ++a)
+        for (int ra = rs[a]; ra < rs[a] + rc[a]; ++ra)
+          for (int bq = 0; bq < ncol; ++bq)
+            for (int cb = cs[bq]; cb < cs[bq] + cc[bq]; ++cb)
+              acc += __ldg(zz + ((long long)(sa - zmin) * He + (ra - amin)) * We + (cb - bmin));
+  x[(long long)bc * D * HW + idx] = acc;
+}
+
+static int run_corr3d(const float* in, const float* filt, float* out, int B, int C, int Din, int Hin, int Win, int Dout, int Hout,
+                      int Wout, int FB, int FC, int d, int h, int w, int flip, int off_z, int off_i, int off_j, int map, void* stream) {
+  Blur3dParams S;
+  S.Din = Din; S.Dout = Dout; S.d = d; S.off_z = off_z;
+  auto layout = [&](int zt, int nbuf, bool align) {
+    S.P = corr_params(C, Hin, Win, Hout, Wout, FB, FC, h, w, flip, off_i, off_j, map, align);
+    S.zt = zt; S.nbuf = nbuf; S.ring = zt + nbuf - 1;
+    return S.ring * filter_bytes(S.P) + nbuf * (patch_bytes(S.P) + 128);
+  };
+  // Layouts, best first: B3_ZT planes double-buffered, then single-buffered, then one plane.  The last holds one filter slice and
+  // one patch, blur_corr_kernel's footprint, so each slice accepts exactly the 2-D filters (unshifted at the budget line, as there).
+  bool aligned = true;
+  size_t smem = layout(B3_ZT, 2, true);
+  if (smem > BL_SMEM_BUDGET) smem = layout(B3_ZT, 1, true);
+  if (smem > BL_SMEM_BUDGET) smem = layout(1, 1, true);
+  if (smem > BL_SMEM_BUDGET && S.P.shift) {
+    smem = layout(1, 1, false);
+    aligned = false;
+  }
+  if (smem > BL_SMEM_BUDGET) return set_error(DINVK_EUNSUPPORTED, "blur3d: filter slice %dx%d too large for the tiled kernel", h, w);
+  S.ntiles = S.P.tiles_x * ceil_div(Hout, BL_T);
+  const long long groups = ceil_div(Dout, S.zt), ctas = (long long)S.ntiles * groups;
+  if ((long long)B * C > 65535 || ctas > 2147483647LL) return set_error(DINVK_EINVAL, "blur3d: grid too large");
+  int rc = allow_smem(blur3d_corr_kernel, smem);
+  if (rc) return rc;
+  tt::TileMap tmap = tt::TileMap();
+  int use_tma = 0;
+#ifndef DINVK_EMUL
+  if (aligned && (long long)B * C * Din <= 2147483647LL && !getenv("DINVK_NO_TMA_STAGING"))
+    use_tma = tt::make_map_f32(&tmap, in, Win, Hin, B * C * Din, S.P.PW, BL_T + h - 1) ? 1 : 0;
+#endif
+  DINVK_LAUNCH(blur3d_corr_kernel, dim3((unsigned)ctas, B * C), dim3(256), smem, stream, tmap, use_tma, in, filt, out, S);
+  return DINVK_POST_LAUNCH();
+}
+
+static int check_blur3d_args(const void* a, const void* f, const void* o, int B, int C, int D, int H, int W, int FB, int FC, int d,
+                             int h, int w, int padding) {
+  DINVK_CHECK_ARG(a && f && o, "blur3d: null pointer");
+  DINVK_CHECK_ARG(B >= 0 && C >= 1 && D >= 1 && H >= 1 && W >= 1 && d >= 1 && h >= 1 && w >= 1, "blur3d: bad shape");
+  DINVK_CHECK_ARG((FB == 1 || FB == B) && (FC == 1 || FC == C), "blur3d: filter batch/channel (%d,%d) must be 1 or match (%d,%d)", FB, FC, B, C);
+  DINVK_CHECK_ARG(padding >= DINVK_PAD_VALID && padding <= DINVK_PAD_CONSTANT, "blur3d: unknown padding %d", padding);
+  DINVK_CHECK_ARG(padding != DINVK_PAD_VALID || (D >= d && H >= h && W >= w),
+                  "blur3d: valid padding needs a volume at least as large as the filter");
+  DINVK_CHECK_ARG(padding != DINVK_PAD_REFLECT || (d / 2 < D && h / 2 < H && w / 2 < W), "blur3d: reflect padding needs pad < volume size");
+  return 0;
+}
+
 }  // namespace dinvk
 
 using namespace dinvk;
@@ -837,4 +1130,49 @@ extern "C" int dinvk_tiled_svblur_fwd(const float* x, const float* mult, const f
 extern "C" int dinvk_tiled_svblur_adj(const float* y, const float* mult, const float* filt, float* x, int B, int C, int H, int W,
                                       int FB, int FC, int K, int h, int w, int P1, int P2, int s1, int s2, void* stream) {
   return tiled_svblur(false, y, mult, filt, x, B, C, H, W, FB, FC, K, h, w, P1, P2, s1, s2, stream);
+}
+
+// ---- 3-D blur: deepinv/physics/functional/convolution.py:333-438 (conv3d / conv_transpose3d: flip + F.pad + grouped F.conv3d,
+// and F.conv_transpose3d + _apply_transpose_padding :689-758), the bodies of Blur.A / A_adjoint on (B, C, D, H, W) volumes
+// (deepinv/physics/blur.py:496-561) ---------------------------------------------------------------------------------------------
+extern "C" int dinvk_blur3d_fwd(const float* x, const float* filt, float* y, int B, int C, int D, int H, int W, int FB, int FC, int d,
+                                int h, int w, int padding, void* stream) {
+  int rc = check_blur3d_args(x, filt, y, B, C, D, H, W, FB, FC, d, h, w, padding);
+  if (rc) return rc;
+  if (B == 0) return DINVK_OK;
+  if (padding == DINVK_PAD_VALID)
+    return run_corr3d(x, filt, y, B, C, D, H, W, D - d + 1, H - h + 1, W - w + 1, FB, FC, d, h, w, 1, 0, 0, 0, 0, stream);
+  const int map = padding == DINVK_PAD_CIRCULAR ? 1 : padding == DINVK_PAD_REPLICATE ? 2 : padding == DINVK_PAD_REFLECT ? 3 : 0;
+  return run_corr3d(x, filt, y, B, C, D, H, W, D, H, W, FB, FC, d, h, w, 1, d / 2 - (d - 1), h / 2 - (h - 1), w / 2 - (w - 1), map,
+                    stream);
+}
+
+extern "C" size_t dinvk_blur3d_adj_workspace_bytes(int B, int C, int D, int H, int W, int d, int h, int w, int padding) {
+  if (padding == DINVK_PAD_REPLICATE || padding == DINVK_PAD_REFLECT)
+    return sizeof(float) * (size_t)B * C * (size_t)(D + d - 1) * (size_t)(H + h - 1) * (size_t)(W + w - 1) + 256;
+  return 256;
+}
+
+extern "C" int dinvk_blur3d_adj(const float* y, const float* filt, float* x, int B, int C, int D, int H, int W, int FB, int FC, int d,
+                                int h, int w, int padding, void* workspace, size_t workspace_bytes, void* stream) {
+  int rc = check_blur3d_args(y, filt, x, B, C, D, H, W, FB, FC, d, h, w, padding);
+  if (rc) return rc;
+  if (B == 0) return DINVK_OK;
+  if (padding == DINVK_PAD_VALID)
+    return run_corr3d(y, filt, x, B, C, D - d + 1, H - h + 1, W - w + 1, D, H, W, FB, FC, d, h, w, 0, -(d - 1), -(h - 1), -(w - 1), 0,
+                      stream);
+  if (padding == DINVK_PAD_CIRCULAR || padding == DINVK_PAD_CONSTANT)
+    return run_corr3d(y, filt, x, B, C, D, H, W, D, H, W, FB, FC, d, h, w, 0, -(d / 2), -(h / 2), -(w / 2),
+                      padding == DINVK_PAD_CIRCULAR ? 1 : 0, stream);
+  // replicate / reflect: zero-extended correlation onto the (D+d-1, H+h-1, W+w-1) volume, then fold it back
+  const size_t need = dinvk_blur3d_adj_workspace_bytes(B, C, D, H, W, d, h, w, padding);
+  if (!workspace || workspace_bytes < need) return set_error(DINVK_EWORKSPACE, "dinvk_blur3d_adj: workspace %zu < %zu", workspace_bytes, need);
+  float* z = reinterpret_cast<float*>(((uintptr_t)workspace + 127) & ~(uintptr_t)127);
+  const int De = D + d - 1, He = H + h - 1, We = W + w - 1;
+  if ((rc = run_corr3d(y, filt, z, B, C, D, H, W, De, He, We, FB, FC, d, h, w, 0, -(d - 1), -(h - 1), -(w - 1), 0, stream))) return rc;
+  const long long blocks = ((long long)D * H * W + 255) / 256;
+  if (blocks > 2147483647LL) return set_error(DINVK_EINVAL, "blur3d: grid too large");
+  DINVK_LAUNCH(blur3d_fold_kernel, dim3((unsigned)blocks, B * C), dim3(256), 0, stream, (const float*)z, x, D, H, W, d, h, w,
+               padding == DINVK_PAD_REPLICATE ? 2 : 3);
+  return DINVK_POST_LAUNCH();
 }

@@ -417,6 +417,39 @@ def blur_adj(y, filt, padding: int, H: int, W: int) -> torch.Tensor:
     return x
 
 
+def blur3d_fwd(x, filt, padding: int) -> torch.Tensor:
+    """the 3-D blur of (B,C,D,H,W) volumes by (FB,FC,d,h,w) filters (csrc/blur.cu: blur3d_corr_kernel)"""
+    dev = _require_cuda(x, filt)
+    x, filt = _f32c(x), _f32c(filt)
+    B, C, D, H, W = x.shape
+    FB, FC, d, h, w = filt.shape
+    shape = (B, C, D - d + 1, H - h + 1, W - w + 1) if padding == _ffi.PAD_VALID else (B, C, D, H, W)
+    if min(shape[2:]) < 1:  # a volume smaller than the filter: the library's argument check raises
+        check(get_lib().dinvk_blur3d_fwd(_p(x), _p(filt), _p(x), B, C, D, H, W, FB, FC, d, h, w, padding, _stream(dev)))
+    y = torch.empty(shape, dtype=torch.float32, device=dev)
+    if y.numel() == 0:
+        return y
+    check(get_lib().dinvk_blur3d_fwd(_p(x), _p(filt), _p(y), B, C, D, H, W, FB, FC, d, h, w, padding, _stream(dev)))
+    return y
+
+
+def blur3d_adj(y, filt, padding: int, D: int, H: int, W: int) -> torch.Tensor:
+    """the transpose of blur3d_fwd onto a (B,C,D,H,W) volume"""
+    dev = _require_cuda(y, filt)
+    y, filt = _f32c(y), _f32c(filt)
+    B, C = y.shape[:2]
+    FB, FC, d, h, w = filt.shape
+    x = torch.empty(B, C, D, H, W, dtype=torch.float32, device=dev)
+    if x.numel() == 0:
+        return x
+    lib = get_lib()
+    nb = lib.dinvk_blur3d_adj_workspace_bytes(B, C, D, H, W, d, h, w, padding)
+    ws = workspace(dev, nb, "blur")
+    check(lib.dinvk_blur3d_adj(_p(y), _p(filt), _p(x), B, C, D, H, W, FB, FC, d, h, w, padding, _p(ws), ws.numel(),
+                               _stream(dev)))
+    return x
+
+
 def _svblur_shapes(mult, filt, B: int, C: int, H: int, W: int):
     MB, MC, K, Hm, Wm = mult.shape
     FB, FC, Kf, h, w = filt.shape

@@ -2,7 +2,8 @@
 
 Drop-in for deepinv/physics/blur.py:443-737.  `Blur.A / A_adjoint` call `dinvk_blur_fwd / _adj`
 (csrc/blur.cu: all five paddings resolved in index space, per-sample / per-channel filters as in
-convolution.py:761-787); `use_fft=True` routes the circular case through the spectral kernels.
+convolution.py:761-787), and `dinvk_blur3d_fwd / _adj` on (B,C,D,H,W) volumes; `use_fft=True` routes
+the circular case through the spectral kernels.
 `BlurFFT` keeps the reference's buffers (`filter`, `mask` = |h^| duplicated on a trailing axis, `angle`)
 and its rfft2-domain U/V methods, but A / A_adjoint / A_adjoint_A / prox_l2 / A_dagger are single
 fused launches of `dinvk_spectral` on PAIRS of real images packed as one complex image (a real
@@ -40,7 +41,12 @@ def _check_filter(filt: Tensor, B: int, C: int) -> None:
 
 
 class Blur(LinearPhysics):
-    r"""y = w * x (blur.py:443-561)"""
+    r"""y = w * x (blur.py:443-561), on (B, C, H, W) images with (b, c, h, w) filters or on (B, C, D, H, W) volumes with
+    (b, c, d, h, w) filters, b in {1, B}, c in {1, C}, all five paddings in both ranks.
+
+    On volumes the direct kernel (`dinvk_blur3d_fwd / _adj`) runs for both values of ``use_fft``: the flag is stored as in
+    the reference, where it selects FFT convolutions, the same operator up to rounding.  `A_dagger`, `prox_l2` and the norm
+    estimate of a 3-D blur are the CG / power-method versions of LinearPhysics."""
 
     def __init__(self, filter: Tensor = None, padding: str = "valid", use_fft: bool = False, device="cpu", **kwargs):
         super().__init__(device=device, **kwargs)
@@ -56,8 +62,10 @@ class Blur(LinearPhysics):
 
     def A(self, x: Tensor, filter: Tensor = None, **kwargs) -> Tensor:
         self.update_parameters(filter=filter, **kwargs)
+        if x.dim() == 5:
+            return self._A3d(x)
         if x.dim() != 4:
-            raise ValueError(f"Expected Tensor dimension to be 4 (2-D blur), is {x.dim()}")
+            raise ValueError(f"Expected Tensor dimension to be 4 or 5, is {x.dim()}")
         if self.filter.dim() != 4:
             raise ValueError("Input and filter must be 4D tensors")
         _check_filter(self.filter, x.shape[0], x.shape[1])
@@ -67,13 +75,35 @@ class Blur(LinearPhysics):
 
     def A_adjoint(self, y: Tensor, filter: Tensor = None, **kwargs) -> Tensor:
         self.update_parameters(filter=filter, **kwargs)
+        if y.dim() == 5:
+            return self._At3d(y)
         if y.dim() != 4:
-            raise ValueError(f"Expected Tensor dimension to be 4 (2-D blur), is {y.dim()}")
+            raise ValueError(f"Expected Tensor dimension to be 4 or 5, is {y.dim()}")
         _check_filter(self.filter, y.shape[0], y.shape[1])
         code = _padding_code(self.padding)
         h, w = self.filter.shape[-2:]
         H, W = (y.shape[-2] + h - 1, y.shape[-1] + w - 1) if code == _ffi.PAD_VALID else y.shape[-2:]
         return linear_apply(y, lambda t: ops.blur_adj(t, self.filter, code, H, W), self._fwd)
+
+    # 3-D: convolution.py:333-438 (conv3d / conv_transpose3d) on dinvk_blur3d_fwd / _adj
+    def _filter3d(self, t: Tensor) -> int:
+        if self.filter.dim() != 5:
+            raise ValueError("Input and filter must be 5D tensors")
+        _check_filter(self.filter, t.shape[0], t.shape[1])
+        return _padding_code(self.padding)
+
+    def _A3d(self, x: Tensor) -> Tensor:
+        code = self._filter3d(x)
+        D, H, W = x.shape[-3:]
+        return linear_apply(x, lambda t: ops.blur3d_fwd(t, self.filter, code),
+                            lambda t: ops.blur3d_adj(t, self.filter, code, D, H, W))
+
+    def _At3d(self, y: Tensor) -> Tensor:
+        code = self._filter3d(y)
+        d, h, w = self.filter.shape[-3:]
+        D, H, W = (y.shape[-3] + d - 1, y.shape[-2] + h - 1, y.shape[-1] + w - 1) if code == _ffi.PAD_VALID else y.shape[-3:]
+        return linear_apply(y, lambda t: ops.blur3d_adj(t, self.filter, code, D, H, W),
+                            lambda t: ops.blur3d_fwd(t, self.filter, code))
 
     def update_parameters(self, filter: Tensor = None, **kwargs):
         if filter is not None and self.filter is None:

@@ -218,6 +218,20 @@ int dinvk_blur_adj(const float* y, const float* filt, float* x, int B, int C, in
                    int FB, int FC, int h, int w, int padding,
                    void* workspace, size_t workspace_bytes, void* stream);
 
+/* 3-D blur (deepinv/physics/functional/convolution.py:333-438 conv3d / conv_transpose3d with _apply_transpose_padding
+ * :689-758; deepinv/physics/blur.py:496-561, Blur.A / A_adjoint on 5-D tensors).
+ * x (B,C,D,H,W), filter (FB,FC,d,h,w) with FB in {1,B}, FC in {1,C}; paddings as dinvk_blur_fwd, applied per axis with the same
+ * origin (d/2, h/2, w/2).  fwd output is (B,C,D-d+1,H-h+1,W-w+1) for valid else (B,C,D,H,W); adj input is that shape, output
+ * (B,C,D,H,W).  h and w are limited as in dinvk_blur_fwd (DINVK_EUNSUPPORTED past it), d is not.  One launch (two for the
+ * replicate / reflect adjoint), no atomics. */
+int dinvk_blur3d_fwd(const float* x, const float* filt, float* y, int B, int C, int D, int H, int W,
+                     int FB, int FC, int d, int h, int w, int padding, void* stream);
+/* transpose; replicate/reflect need a workspace for the zero-extended (D+d-1, H+h-1, W+w-1) volume that is folded back */
+size_t dinvk_blur3d_adj_workspace_bytes(int B, int C, int D, int H, int W, int d, int h, int w, int padding);
+int dinvk_blur3d_adj(const float* y, const float* filt, float* x, int B, int C, int D, int H, int W,
+                     int FB, int FC, int d, int h, int w, int padding,
+                     void* workspace, size_t workspace_bytes, void* stream);
+
 /* Space-varying blur, the product convolution y = sum_{k<K} h_k * (w_k . x) and its adjoint
  * x = sum_k w_k . (h_k^T * y) (deepinv/physics/functional/product_convolution.py:10-68).
  * x (B,C,H,W), multipliers (MB,MC,K,H,W), filters (FB,FC,K,h,w); MB, FB in {1,B} and MC, FC in {1,C}
