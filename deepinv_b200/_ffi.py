@@ -36,6 +36,8 @@ _SIGNATURES = {
     "dinvk_spectral_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "dinvk_spectral": (c_int, [C.POINTER(SpectralArgs), c_void_p, c_size_t, c_void_p]),
     "dinvk_fft_prepare": (c_int, [c_int, c_int]),
+    "dinvk_spectral3d_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
+    "dinvk_spectral3d": (c_int, [C.POINTER(SpectralArgs), c_int, c_void_p, c_size_t, c_void_p]),
     "dinvk_ramp_filter_workspace_bytes": (c_size_t, [c_int, c_int]),
     "dinvk_ramp_filter": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_size_t, c_void_p]),
     "dinvk_axpbypcz": (c_int, [c_void_p, c_void_p, c_float, c_void_p, c_float, c_void_p, c_float, c_int64, c_void_p]),

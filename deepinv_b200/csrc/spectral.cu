@@ -710,6 +710,179 @@ extern "C" int dinvk_spectral(const dinvk_spectral_args* ap, void* workspace, si
 }
 
 // ---------------------------------------------------------------------------------------------
+// 3-D: the same contract on contiguous (D,H,W) volumes.  Every axis is a pass of the 2-D family over its own view of the
+// same memory, so the 3-D operator issues no copy and no permute:
+//   depth  COL pass over one (D, H*W) "image" per volume: a CTA owns a strip of consecutive (h,w) columns and all D planes,
+//          so its global accesses are the column pass's coalesced row segments; the coil maps (batch|1, ncoil, D, H, W) are
+//          (ncoil, D, H*W) images in this view, which is where the forward operator multiplies by them;
+//   H      COL pass over the B*D slices (H, W) of the interleaved workspace;
+//   W      ROW pass over one (D*H, W) "image" per volume: the planar (batch,2,ncoil,D,H,W) layout and the multiplier
+//          mask[b*sb + ch*sc + (d*H + h)*sh + w] are the 2-D addressing with D*H rows, so the mask is applied here.
+// ---------------------------------------------------------------------------------------------
+extern "C" size_t dinvk_spectral3d_workspace_bytes(int B, int D, int H, int W) {
+  return 2 * (size_t)B * (size_t)D * (size_t)H * (size_t)W * sizeof(float2) + 256;
+}
+
+extern "C" int dinvk_spectral3d(const dinvk_spectral_args* ap, int D, void* workspace, size_t workspace_bytes, void* stream) {
+  DINVK_CHECK_ARG(ap != nullptr, "dinvk_spectral3d: null args");
+  const dinvk_spectral_args& a = *ap;
+  DINVK_CHECK_ARG(a.B >= 0 && D >= 1 && a.H >= 1 && a.W >= 1, "dinvk_spectral3d: bad shape B=%d D=%d H=%d W=%d", a.B, D, a.H, a.W);
+  const long long vol = (long long)D * a.H * a.W;
+  DINVK_CHECK_ARG(vol < (1LL << 31), "dinvk_spectral3d: a volume of D*H*W = %lld elements (D=%d H=%d W=%d) exceeds 2^31 - 1", vol, D,
+                  a.H, a.W);
+  DINVK_CHECK_ARG((long long)a.B * D < (1LL << 31), "dinvk_spectral3d: B*D = %lld slices exceeds 2^31 - 1", (long long)a.B * D);
+  DINVK_CHECK_ARG(a.p0 && a.out, "dinvk_spectral3d: p0/out must not be null");
+  DINVK_CHECK_ARG(a.gmode >= DINVK_G_NONE && a.gmode <= DINVK_G_CMUL_CONJ, "dinvk_spectral3d: bad gmode %d", a.gmode);
+  DINVK_CHECK_ARG(a.gmode == DINVK_G_NONE || a.mask, "dinvk_spectral3d: gmode %d needs a mask", a.gmode);
+  const bool coils = a.coil_mode != 0;
+  const int nc = coils ? a.ncoil : std::max(a.ncoil, 1);  // coil_mode 0: ncoil planar volumes per sample, no maps
+  if (coils) {
+    DINVK_CHECK_ARG(a.coil_mode >= 1 && a.coil_mode <= 3, "dinvk_spectral3d: bad coil_mode %d", a.coil_mode);
+    DINVK_CHECK_ARG(nc >= 1, "dinvk_spectral3d: coil_mode %d needs ncoil >= 1, got %d", a.coil_mode, nc);
+    DINVK_CHECK_ARG(a.B % nc == 0, "dinvk_spectral3d: B=%d not a multiple of ncoil=%d", a.B, nc);
+    DINVK_CHECK_ARG(a.coil_mode == 3 || a.coil_maps, "dinvk_spectral3d: coil maps missing");
+    DINVK_CHECK_ARG(!(a.coil_mode == 1) || (a.fwd && !a.inv), "dinvk_spectral3d: coil_mode 1 is the forward operator");
+    DINVK_CHECK_ARG(!(a.coil_mode >= 2) || (!a.fwd && a.inv), "dinvk_spectral3d: coil_mode 2/3 is the adjoint operator");
+    DINVK_CHECK_ARG(!(a.coil_mode >= 2) || (!a.q0 && !a.q1), "dinvk_spectral3d: epilogue terms unsupported with coil reduction");
+  } else {
+    DINVK_CHECK_ARG(a.B % nc == 0, "dinvk_spectral3d: B=%d not a multiple of ncoil=%d", a.B, nc);
+  }
+  if (a.B == 0) return DINVK_OK;
+  const size_t need = dinvk_spectral3d_workspace_bytes(a.B, D, a.H, a.W);
+  DINVK_CHECK_ARG(workspace != nullptr || (!a.fwd && !a.inv), "dinvk_spectral3d: workspace is null");
+  if (workspace_bytes < need && (a.fwd || a.inv)) return set_error(DINVK_EWORKSPACE, "dinvk_spectral3d: workspace %zu < %zu", workspace_bytes, need);
+  const int HW = a.H * a.W;
+  uintptr_t wsp = ((uintptr_t)workspace + 127) & ~(uintptr_t)127;
+  float2* T1 = reinterpret_cast<float2*>(wsp);
+  float2* T2 = T1 + (size_t)a.B * vol;
+  const bool coil_reduce = coils && a.coil_mode >= 2;
+
+  Tables tD, tH, tW;
+  FftPlan pD = FftPlan(), pH = FftPlan(), pW = FftPlan();
+  int rc;
+  const int cen = a.centered ? 1 : 0;
+  if ((rc = get_tables(D, cen, &tD))) return rc;
+  if ((rc = get_tables(a.H, cen, &tH))) return rc;
+  if ((rc = get_tables(a.W, cen, &tW))) return rc;
+  TileCfg dcfg, hcfg, wcfg;
+  const bool okD = make_fft_plan(D, &pD), okH = make_fft_plan(a.H, &pH), okW = make_fft_plan(a.W, &pW);  // all initialised
+  // an axis runs as a tile pass when its plan and tile fit; the fused paths below need all three
+  const bool tileD = okD && col_cfg(pD, D, HW, &dcfg);
+  const bool tileH = okH && col_cfg(pH, a.H, a.W, &hcfg);
+  const bool tileW = okW && row_cfg(pW, a.W, &wcfg);
+  const bool fast = tileD && tileH && tileW;
+
+  // pass parameters on one of the three views; the source / destination are the user's planar tensors or a workspace
+  PassParams P;
+  auto depth = [&]() { init_pass(P, a); P.B = a.B; P.H = D; P.W = HW; P.wv = HW; set_axis(P, tD, pD); };
+  auto slice = [&]() { init_pass(P, a); P.B = a.B * D; P.H = a.H; P.W = a.W; P.wv = a.W; set_axis(P, tH, pH); };
+  auto rows = [&]() { init_pass(P, a); P.B = a.B; P.H = D * a.H; P.W = a.W; P.wv = a.W; set_axis(P, tW, pW); };
+  auto source = [&]() {
+    P.p0 = a.p0; P.p1 = a.p1; P.a0 = a.a0; P.a1 = a.p1 ? a.a1 : 0.f;
+    if (a.coil_mode == 1) { P.src_div = nc; P.coil = reinterpret_cast<const float2*>(a.coil_maps); P.coil_sb = a.coil_sb; }
+    else P.src_nc = nc;
+  };
+  auto dest = [&](float2* ws) {
+    if (ws) { P.tout = ws; return; }
+    P.out = a.out; P.q0 = a.q0; P.q1 = a.q1; P.e0 = a.e0; P.e1 = a.q0 ? a.e1 : 0.f; P.e2 = a.q1 ? a.e2 : 0.f;
+    P.dst_nc = a.coil_mode <= 1 ? nc : 1;
+  };
+  TileCfg ecfg; ecfg.nthr = 256; ecfg.lines = std::max(1, 4096 / a.W); ecfg.smem = (size_t)ecfg.lines * row_line_stride(a.W) * sizeof(float2);
+
+  if (!a.fwd && !a.inv) {  // pure elementwise
+    rows(); source(); set_mult(P, a, true); dest(nullptr);
+    return launch_pass(false, P, ecfg, stream);
+  }
+  float2* red = nullptr;  // interleaved per-coil volumes for the coil reduction
+  if (fast) {
+    if (a.fwd && !a.inv) {
+      // A: depth(fwd, coil maps) planar -> T1 ; H(fwd) T1 -> T2 ; W(fwd, multiplier) T2 -> out
+      depth(); source(); P.dir1 = -1; P.tout = T1;
+      if ((rc = launch_pass(true, P, dcfg, stream))) return rc;
+      slice(); P.tin = T1; P.dir1 = -1; P.tout = T2;
+      if ((rc = launch_pass(true, P, hcfg, stream))) return rc;
+      rows(); P.tin = T2; P.dir1 = -1; set_mult(P, a, false); dest(nullptr);
+      return launch_pass(false, P, wcfg, stream);
+    }
+    if (!a.fwd && a.inv) {
+      // A^T: W(multiplier at load, inv) planar -> T1 ; H(inv) T1 -> T2 ; depth(inv) T2 -> out (or T1 for the coil reduction)
+      rows(); source(); set_mult(P, a, true); P.dir1 = +1; P.tout = T1;
+      if ((rc = launch_pass(false, P, wcfg, stream))) return rc;
+      slice(); P.tin = T1; P.dir1 = +1; P.tout = T2;
+      if ((rc = launch_pass(true, P, hcfg, stream))) return rc;
+      red = coil_reduce ? T1 : nullptr;
+      depth(); P.tin = T2; P.dir1 = +1; dest(red);
+      if ((rc = launch_pass(true, P, dcfg, stream))) return rc;
+    } else {
+      // A^T A / prox / data step: depth, H, W(fwd, multiplier, inv), H, depth(epilogue)
+      depth(); source(); P.dir1 = -1; P.tout = T1;
+      if ((rc = launch_pass(true, P, dcfg, stream))) return rc;
+      slice(); P.tin = T1; P.dir1 = -1; P.tout = T2;
+      if ((rc = launch_pass(true, P, hcfg, stream))) return rc;
+      rows(); P.tin = T2; P.dir1 = -1; P.dir2 = +1; set_mult(P, a, false); P.tout = T1;
+      if ((rc = launch_pass(false, P, wcfg, stream))) return rc;
+      slice(); P.tin = T1; P.dir1 = +1; P.tout = T2;
+      if ((rc = launch_pass(true, P, hcfg, stream))) return rc;
+      depth(); P.tin = T2; P.dir1 = +1; dest(nullptr);
+      return launch_pass(true, P, dcfg, stream);
+    }
+  } else {
+    // an axis with a prime factor above 5 (or beyond the tile budget): elementwise prologue -> one transform per axis on the
+    // interleaved workspace (a tile pass where the axis allows one, else the O(N^2) DFT) -> elementwise epilogue (or the
+    // coil reduction)
+    const long long total = (long long)a.B * vol;
+    const dim3 ngrid((unsigned)ceil_div(total, 256));
+    float2 *cur = T1, *oth = T2;
+    auto axis = [&](int ax, int dir) -> int {  // ax 0 depth, 1 H, 2 W
+      const bool tile = ax == 0 ? tileD : ax == 1 ? tileH : tileW;
+      int r = 0;
+      if (tile) {
+        if (ax == 0) depth(); else if (ax == 1) slice(); else rows();
+        P.tin = cur; P.tout = oth; P.dir1 = dir;
+        r = launch_pass(ax != 2, P, ax == 0 ? dcfg : ax == 1 ? hcfg : wcfg, stream);
+      } else if (ax == 0) {
+        DINVK_LAUNCH(dft_axis_naive_kernel, ngrid, dim3(256), 0, stream, cur, oth, a.B, D, HW, 0, dir, cen, tD.tw);
+      } else {
+        DINVK_LAUNCH(dft_axis_naive_kernel, ngrid, dim3(256), 0, stream, cur, oth, a.B * D, a.H, a.W, ax == 2 ? 1 : 0, dir, cen,
+                     ax == 2 ? tW.tw : tH.tw);
+      }
+      std::swap(cur, oth);
+      return r;
+    };
+    rows(); source(); if (!a.fwd) set_mult(P, a, true); P.tout = cur;
+    if ((rc = launch_pass(false, P, ecfg, stream))) return rc;
+    if (a.fwd) {
+      for (int ax = 0; ax < 3; ++ax)
+        if ((rc = axis(ax, -1))) return rc;
+      if ((rc = DINVK_POST_LAUNCH())) return rc;
+      if (a.inv) {  // multiplier in the middle
+        rows(); P.tin = cur; set_mult(P, a, true); P.tout = oth;
+        if ((rc = launch_pass(false, P, ecfg, stream))) return rc;
+        std::swap(cur, oth);
+      }
+    }
+    if (a.inv) {
+      for (int ax = 2; ax >= 0; --ax)
+        if ((rc = axis(ax, +1))) return rc;
+      if ((rc = DINVK_POST_LAUNCH())) return rc;
+    }
+    if (coil_reduce) {
+      red = cur;
+    } else {
+      rows(); P.tin = cur; if (a.fwd && !a.inv) set_mult(P, a, true); dest(nullptr);
+      return launch_pass(false, P, ecfg, stream);
+    }
+  }
+  if (!red) return DINVK_OK;
+  // coil reduction: out[b] = e0 sum_n conj(S[b,n]) v[b,n] (coil_mode 2) or sqrt(sum_n |v[b,n]|^2) (coil_mode 3)
+  const int batch = a.B / nc;
+  DINVK_LAUNCH(coil_combine_kernel, dim3((unsigned)ceil_div((long long)batch * vol, 256)), dim3(256), 0, stream,
+               (const float2*)red, reinterpret_cast<const float2*>(a.coil_maps), (long long)a.coil_sb, a.out, batch, nc, vol,
+               a.coil_mode, a.e0);
+  return DINVK_POST_LAUNCH();
+}
+
+// ---------------------------------------------------------------------------------------------
 // ramp filter (FBP): rows of length N zero-padded to L, multiplied by 2*rfft(f) in the Fourier domain.
 // Two real rows are packed as one complex signal (the filter is real and even, so real and imaginary
 // parts filter independently); the ROW pass runs load(+pad) -> FFT -> multiply -> iFFT -> store(crop).

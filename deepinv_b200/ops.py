@@ -170,6 +170,93 @@ def spectral(
     return out
 
 
+def mask_spec3d(mask: torch.Tensor) -> MaskSpec:
+    """mask: (1|B, 2, D, H, W) fp32 as stored by the reference's 3-D MRI operators (`check_mask(three_d=True)`)"""
+    m = _f32c(mask)
+    assert m.dim() == 5 and m.shape[1] == 2, f"mask shape {tuple(m.shape)}"
+    D, H, W = m.shape[-3:]
+    return MaskSpec(m, 2 * D * H * W if m.shape[0] > 1 else 0, D * H * W, W)
+
+
+def spectral3d(
+    p0: torch.Tensor,
+    D: int,
+    H: int,
+    W: int,
+    *,
+    fwd: bool,
+    inv: bool,
+    centered: bool = True,
+    gmode: int = _ffi.G_NONE,
+    mask: Optional[MaskSpec] = None,
+    a0: float = 1.0,
+    p1: Optional[torch.Tensor] = None,
+    a1: float = 0.0,
+    c: float = 0.0,
+    c_batch: Optional[torch.Tensor] = None,
+    q0: Optional[torch.Tensor] = None,
+    e1: float = 0.0,
+    q1: Optional[torch.Tensor] = None,
+    e2: float = 0.0,
+    e0: float = 1.0,
+    ncoil: int = 0,
+    coil_mode: int = 0,
+    coil_maps: Optional[torch.Tensor] = None,
+    out: Optional[torch.Tensor] = None,
+) -> torch.Tensor:
+    """`spectral` on planar (B,2,...,D,H,W) volumes with the 3-D DFT over the last three dims.  coil_mode 1 / 2 / 3 work for any
+    ncoil >= 1: x (batch,2,D,H,W) -> y (batch,2,ncoil,D,H,W), y -> x, y -> rss (batch,1,D,H,W); maps (1|batch, ncoil, D, H, W)
+    complex64.  Without coils, the dims between the planes and the volume (e.g. the coils of a (B,2,N,D,H,W) k-space) are
+    transformed volume by volume, with the mask of their sample."""
+    dev = _require_cuda(p0, p1, q0, q1, c_batch, coil_maps, None if mask is None else mask.tensor)
+    p0 = _f32c(p0)
+    p1, q0, q1, c_batch = _f32c(p1), _f32c(q0), _f32c(q1), _f32c(c_batch)
+    vol = D * H * W
+    if coil_mode:
+        nc = max(int(ncoil), 1)
+        batch = p0.shape[0]
+        nimg = batch * nc
+        out_shape = {1: (batch, 2, nc, D, H, W), 2: (batch, 2, D, H, W), 3: (batch, 1, D, H, W)}[coil_mode]
+    else:  # (B,2,...,D,H,W): the dims between the planes and the volume are a stack of volumes per sample (ncoil of the ABI)
+        if p0.dim() < 5 or p0.shape[1] != 2 or tuple(p0.shape[-3:]) != (D, H, W):
+            raise ValueError(f"spectral3d: expected a planar (B,2,...,{D},{H},{W}) tensor, got {tuple(p0.shape)}")
+        nc = 1
+        for s in p0.shape[2:-3]:
+            nc *= int(s)
+        nimg = p0.shape[0] * nc
+        out_shape = tuple(p0.shape)
+    if out is None:
+        out = torch.empty(out_shape, dtype=torch.float32, device=dev)
+    else:
+        assert out.is_contiguous() and out.dtype == torch.float32 and tuple(out.shape) == tuple(out_shape)
+    if out.numel() == 0:  # empty batch: nothing to launch (an empty tensor has a null data pointer)
+        return out
+    a = _ffi.SpectralArgs()
+    a.B, a.H, a.W = nimg, H, W
+    a.fwd, a.inv, a.centered, a.gmode = int(fwd), int(inv), int(centered), gmode
+    a.p0, a.p1, a.a0, a.a1 = p0.data_ptr(), (p1.data_ptr() if p1 is not None else None), a0, a1
+    if gmode != _ffi.G_NONE:
+        if mask is None:
+            raise DinvkError("spectral3d: gmode needs a mask")
+        a.mask, a.mask_sb, a.mask_sc, a.mask_sh = mask.tensor.data_ptr(), mask.sb, mask.sc, mask.sh
+    a.c = c
+    a.c_batch = c_batch.data_ptr() if c_batch is not None else None
+    a.q0, a.q1 = (q0.data_ptr() if q0 is not None else None), (q1.data_ptr() if q1 is not None else None)
+    a.e0, a.e1, a.e2 = e0, e1, e2
+    a.out = out.data_ptr()
+    a.ncoil, a.coil_mode = (nc if nc > 1 or coil_mode else 0), coil_mode
+    if coil_maps is not None:
+        cm = coil_maps if coil_maps.is_contiguous() else coil_maps.contiguous()
+        assert cm.dtype == torch.complex64
+        a.coil_maps = cm.data_ptr()
+        a.coil_sb = nc * vol if cm.shape[0] > 1 else 0
+    lib = get_lib()
+    nbytes = lib.dinvk_spectral3d_workspace_bytes(nimg, D, H, W)
+    ws = workspace(dev, nbytes, "spectral")
+    check(lib.dinvk_spectral3d(ctypes.byref(a), D, _p(ws), ws.numel(), _stream(dev)))
+    return out
+
+
 def fft_prepare(n: int, centered: bool = True) -> None:
     check(get_lib().dinvk_fft_prepare(n, int(centered)))
 

@@ -1,9 +1,9 @@
 """MRI / MultiCoilMRI on the fused sm_90a spectral kernels.
 
-Drop-in for deepinv/physics/mri.py:11-695 (2-D and 2-D+t: MRI, MultiCoilMRI, DynamicMRI, SequentialMRI; single-coil
-`three_d=True` runs the separable 3-D transform on the 2-D kernels — a correctness-level path; 3-D multi-coil is out of scope).  Same constructor, buffers (`mask`, `coil_maps`), kwargs-store-as-buffer side
-effects and error types.  Every method below is one or two launches of `dinvk_spectral`
-(csrc/spectral.cu); nothing is computed with torch.fft.
+Drop-in for deepinv/physics/mri.py:11-695 (2-D and 2-D+t: MRI, MultiCoilMRI, DynamicMRI, SequentialMRI; `three_d=True`
+volumes for MRI and MultiCoilMRI).  Same constructor, buffers (`mask`, `coil_maps`), kwargs-store-as-buffer side effects and
+error types.  Every method below is one call of `dinvk_spectral` or, on (B,2,D,H,W) volumes, of `dinvk_spectral3d`
+(csrc/spectral.cu); nothing is computed with torch.fft and no volume is permuted.
 """
 from __future__ import annotations
 
@@ -39,34 +39,12 @@ class MRIMixin:
     def from_torch_complex(x: Tensor) -> Tensor:
         return torch.view_as_real(x).moveaxis(-1, 1)
 
-    # centred orthonormal 2-D DFT on planar (B,2,H,W) tensors (mixins.py:158-206)
-    @staticmethod
-    def _transform3(x: Tensor, inverse: bool) -> Tensor:
-        """centred orthonormal 3-D DFT of a planar (B,2,D,H,W) volume, separable on the 2-D kernels: the (H,W) transform with
-        the depth folded into the batch, then the depth transform as 1 x D "images" with depth made the fastest axis (two
-        permute copies around it).  Correctness-level path (the 2-D operators are the tuned ones)."""
-        B, _, D, H, W = x.shape
-        t = x.permute(0, 2, 1, 3, 4).reshape(B * D, 2, H, W)
-        t = ops.spectral(t, H, W, fwd=not inverse, inv=inverse)
-        t = t.reshape(B, D, 2, H, W).permute(0, 3, 4, 2, 1).reshape(B * H * W, 2, 1, D)
-        t = ops.spectral(t, 1, D, fwd=not inverse, inv=inverse)
-        return t.reshape(B, H, W, 2, D).permute(0, 3, 4, 1, 2)
-
+    # centred orthonormal 2-D (three_d: 3-D) DFT on planar (B,2,H,W) / (B,2,D,H,W) tensors (mixins.py:158-206)
     def im_to_kspace(self, x: Tensor, three_d: bool = False) -> Tensor:
-        if three_d:
-            return linear_apply(x, lambda t: MRIMixin._transform3(t, False), lambda t: MRIMixin._transform3(t, True))
-        H, W = x.shape[-2:]
-        f = lambda t: ops.spectral(t, H, W, fwd=True, inv=False)
-        g = lambda t: ops.spectral(t, H, W, fwd=False, inv=True)
-        return linear_apply(x, f, g)
+        return linear_apply(x, lambda t: _dft(t, three_d, False), lambda t: _dft(t, three_d, True))
 
     def kspace_to_im(self, y: Tensor, three_d: bool = False) -> Tensor:
-        if three_d:
-            return linear_apply(y, lambda t: MRIMixin._transform3(t, True), lambda t: MRIMixin._transform3(t, False))
-        H, W = y.shape[-2:]
-        f = lambda t: ops.spectral(t, H, W, fwd=True, inv=False)
-        g = lambda t: ops.spectral(t, H, W, fwd=False, inv=True)
-        return linear_apply(y, g, f)
+        return linear_apply(y, lambda t: _dft(t, three_d, True), lambda t: _dft(t, three_d, False))
 
     def crop(self, x: Tensor, crop: bool = True, shape=None, rescale: bool = False) -> Tensor:
         """centre crop to img_size (mixins.py:208-247)"""
@@ -81,6 +59,10 @@ class MRIMixin:
                                                   antialias=True).reshape(*x.shape[:-2], *crop_size)
         elif crop:
             h, w = x.shape[-2:]
+            ph, pw = max(crop_size[0] - h, 0), max(crop_size[1] - w, 0)
+            if ph or pw:  # torchvision's CenterCrop zero-pads an input smaller than the crop (the smaller half on top / left)
+                x = torch.nn.functional.pad(x, (pw // 2, pw - pw // 2, ph // 2, ph - ph // 2))
+                h, w = x.shape[-2:]
             top = int(round((h - crop_size[0]) / 2.0))
             left = int(round((w - crop_size[1]) / 2.0))
             out = x[..., top: top + crop_size[0], left: left + crop_size[1]]
@@ -100,9 +82,13 @@ class MRIMixin:
         return ss.sqrt()
 
 
-def _no_3d(three_d: bool) -> None:
+def _dft(t: Tensor, three_d: bool, inverse: bool) -> Tensor:
+    """centred orthonormal DFT over the last two (three_d: three) dims of a planar (B,2,...) tensor"""
     if three_d:
-        raise NotImplementedError("deepinv_b200: 3-D multi-coil MRI is outside the accelerated path (SURVEY.md §8); use the reference")
+        if t.dim() < 5 or t.shape[1] != 2:
+            raise ValueError(f"expected a planar (B,2,...,D,H,W) tensor, got {tuple(t.shape)}")
+        return ops.spectral3d(t, *t.shape[-3:], fwd=not inverse, inv=inverse)
+    return ops.spectral(t, *t.shape[-2:], fwd=not inverse, inv=inverse)
 
 
 class _MaskCache:
@@ -112,9 +98,9 @@ class _MaskCache:
         self.key = None
         self.spec = None
 
-    def get(self, mask: Tensor, H: int, W: int) -> ops.MaskSpec:
+    def get(self, mask: Tensor, three_d: bool = False) -> ops.MaskSpec:
         if not cache_hit(self.key, mask):
-            self.spec = ops.mask_spec_from_real(mask, H, W)
+            self.spec = ops.mask_spec3d(mask) if three_d else ops.mask_spec_from_real(mask, mask.shape[-2], mask.shape[-1])
             self.key = TensorKey(mask)
         return self.spec
 
@@ -139,16 +125,21 @@ class MRI(MRIMixin, DecomposablePhysics):
 
     # ---- helpers -------------------------------------------------------------------------------
     def _spec(self) -> ops.MaskSpec:
-        m = self.mask
-        return self._mcache.get(m, m.shape[-2], m.shape[-1])
+        return self._mcache.get(self.mask, self.three_d)
 
-    def _hw(self):
-        return int(self.mask.shape[-2]), int(self.mask.shape[-1])
+    def _dims(self) -> tuple:
+        """(H, W), or (D, H, W) for three_d"""
+        return tuple(int(s) for s in self.mask.shape[(-3 if self.three_d else -2):])
+
+    def _op(self, t: Tensor, fwd: bool, inv: bool, gmode: int, **kw) -> Tensor:
+        """one fused call of the 2-D (three_d: 3-D) spectral entry with this operator's mask"""
+        fn = ops.spectral3d if self.three_d else ops.spectral
+        return fn(t, *self._dims(), fwd=fwd, inv=inv, gmode=gmode, mask=self._spec(), **kw)
 
     def _check(self, t: Tensor):
-        H, W = self._hw()
-        if t.dim() != 4 or t.shape[1] != 2 or t.shape[-2] != H or t.shape[-1] != W:
-            raise ValueError(f"expected a (B,2,{H},{W}) tensor, got {tuple(t.shape)}")
+        dims = self._dims()
+        if t.dim() != 2 + len(dims) or t.shape[1] != 2 or tuple(t.shape[2:]) != dims:
+            raise ValueError(f"expected a (B,2,{','.join(map(str, dims))}) tensor, got {tuple(t.shape)}")
         mb = self.mask.shape[0]
         if mb != 1 and mb != t.shape[0]:
             raise ValueError(f"mask batch {mb} does not match input batch {t.shape[0]}")
@@ -167,26 +158,18 @@ class MRI(MRIMixin, DecomposablePhysics):
 
     # ---- fused operator bodies ---------------------------------------------------------------
     def _A(self, x, gmode=_ffi.G_MASK):
-        H, W = self._hw()
-        return ops.spectral(x, H, W, fwd=True, inv=False, gmode=gmode, mask=self._spec())
+        return self._op(x, True, False, gmode)
 
     def _At(self, y, gmode=_ffi.G_MASK):
-        H, W = self._hw()
-        return ops.spectral(y, H, W, fwd=False, inv=True, gmode=gmode, mask=self._spec())
+        return self._op(y, False, True, gmode)
 
     def A(self, x: Tensor, mask: Tensor = None, **kwargs) -> Tensor:
         self.update_parameters(mask=mask, **kwargs)
-        if self.three_d:  # 3-D volumes: generic SVD bodies (forward.py:1080-1252) on the separable 3-D transform
-            return DecomposablePhysics.A(self, x)
         self._check(x)
         return linear_apply(x, self._A, self._At)
 
     def A_adjoint(self, y: Tensor, mask: Tensor = None, mag: bool = False, crop: bool = False, **kwargs) -> Tensor:
         self.update_parameters(mask=mask, **kwargs)
-        if self.three_d:
-            x = DecomposablePhysics.A_adjoint(self, y)
-            x = self.rss(x, multicoil=False) if mag else x
-            return self.crop(x, crop=crop) if crop else x
         self._check(y)
         x = linear_apply(y, self._At, self._A)
         if mag:
@@ -197,26 +180,18 @@ class MRI(MRIMixin, DecomposablePhysics):
 
     def A_adjoint_A(self, x: Tensor, mask: Tensor = None, **kwargs) -> Tensor:
         self.update_parameters(mask=mask, **kwargs)
-        if self.three_d:
-            return DecomposablePhysics.A_adjoint_A(self, x)
         self._check(x)
-        H, W = self._hw()
-        f = lambda t: ops.spectral(t, H, W, fwd=True, inv=True, gmode=_ffi.G_SQ, mask=self._spec())
+        f = lambda t: self._op(t, True, True, _ffi.G_SQ)
         return linear_apply(x, f, f)
 
     def A_A_adjoint(self, y: Tensor, mask: Tensor = None, **kwargs) -> Tensor:
         self.update_parameters(mask=mask, **kwargs)
-        if self.three_d:
-            return DecomposablePhysics.A_A_adjoint(self, y)
         self._check(y)
-        H, W = self._hw()
-        f = lambda t: ops.spectral(t, H, W, fwd=False, inv=False, gmode=_ffi.G_SQ, mask=self._spec())
+        f = lambda t: self._op(t, False, False, _ffi.G_SQ)
         return linear_apply(y, f, f)
 
     def A_dagger(self, y: Tensor, mask: Tensor = None, **kwargs) -> Tensor:
         self.update_parameters(mask=mask, **kwargs)
-        if self.three_d:
-            return DecomposablePhysics.A_dagger(self, y)
         self._check(y)
         if torch.is_grad_enabled() and y.requires_grad:
             return super().A_dagger(y)
@@ -233,31 +208,24 @@ class MRI(MRIMixin, DecomposablePhysics):
         r"""argmin_x gamma/2 ||Ax-y||^2 + 1/2 ||x-z||^2 = V((V^T(A^T y + z/gamma)) / (s^2 + 1/gamma)) (forward.py:1212-1234)"""
         needs_grad = torch.is_grad_enabled() and (z.requires_grad or y.requires_grad or
                                                   (isinstance(gamma, Tensor) and gamma.requires_grad))
-        if needs_grad or self.three_d:
+        if needs_grad:
             return super().prox_l2(z, y, gamma, **kwargs)
         self._check(z)
-        H, W = self._hw()
         aty = self._cached_At(y)
         if isinstance(gamma, Tensor) and gamma.numel() > 1:
             g = gamma.reshape(-1).to(device=z.device, dtype=torch.float32)
             if g.numel() != z.shape[0]:
                 raise ValueError("per-sample gamma must have one entry per batch element")
-            zg = z / g.reshape(-1, 1, 1, 1)
-            return ops.spectral(aty, H, W, fwd=True, inv=True, gmode=_ffi.G_INV_SQ_PLUS_C, mask=self._spec(),
-                                p1=zg, a1=1.0, c_batch=(1.0 / g).contiguous())
+            zg = z / g.reshape(-1, *([1] * (z.dim() - 1)))
+            return self._op(aty, True, True, _ffi.G_INV_SQ_PLUS_C, p1=zg, a1=1.0, c_batch=(1.0 / g).contiguous())
         g = float(gamma)
-        return ops.spectral(aty, H, W, fwd=True, inv=True, gmode=_ffi.G_INV_SQ_PLUS_C, mask=self._spec(),
-                            p1=z, a1=1.0 / g, c=1.0 / g)
+        return self._op(aty, True, True, _ffi.G_INV_SQ_PLUS_C, p1=z, a1=1.0 / g, c=1.0 / g)
 
     def normal_step(self, x: Tensor, aty: Tensor, gamma: float) -> Tensor:
         r"""fused gradient step of the L2 data term: x - gamma * (A^T A x - A^T y)
         (optim_iterators/pgd.py:137-139 with data_fidelity.py:335-336) in one launch for line masks"""
-        if self.three_d:
-            return x - gamma * (DecomposablePhysics.A_adjoint_A(self, x) - aty)
         self._check(x)
-        H, W = self._hw()
-        return ops.spectral(x, H, W, fwd=True, inv=True, gmode=_ffi.G_SQ, mask=self._spec(),
-                            e0=-gamma, q0=x, e1=1.0, q1=aty, e2=gamma)
+        return self._op(x, True, True, _ffi.G_SQ, e0=-gamma, q0=x, e1=1.0, q1=aty, e2=gamma)
 
     def noise(self, x, **kwargs):
         return self.U(self.noise_model(x, **kwargs) * self.mask)
@@ -421,18 +389,19 @@ class SequentialMRI(DynamicMRI):
 
 class MultiCoilMRI(MRIMixin, LinearPhysics):
     r"""y_n = M F (S_n x) (mri.py:166-497); coil multiply, FFT and mask are one fused two-pass launch,
-    the adjoint's coil combination is fused after the inverse transform."""
+    the adjoint's coil combination is fused after the inverse transform.  With three_d=True x is (B,2,D,H,W), y
+    (B,2,N,D,H,W) and every method runs on `dinvk_spectral3d` for any N >= 1; `A_adjoint(rss=True)` returns the RSS volume
+    (B,1,D,H,W), where the reference raises ValueError (its `rss` call omits three_d)."""
 
     def __init__(self, mask: Tensor | None = None, coil_maps: Tensor | int | None = None,
                  img_size: tuple | None = (320, 320), three_d: bool = False, device="cpu", **kwargs):
         super().__init__(device=device, **kwargs)
-        _no_3d(three_d)
         self.img_size = img_size
         self.three_d = three_d
         if mask is None:
             mask = torch.ones(*img_size, device=device)
         if coil_maps is None:
-            coil_maps = torch.ones(self.img_size[-2:], dtype=torch.complex64, device=device)
+            coil_maps = torch.ones(self.img_size[-3:] if three_d else self.img_size[-2:], dtype=torch.complex64, device=device)
         elif isinstance(coil_maps, int):
             raise ImportError("sigpy is required to simulate coil maps; pass a complex64 tensor of maps instead")
         self.register_buffer("mask", self.check_mask(mask, three_d=three_d))
@@ -450,16 +419,30 @@ class MultiCoilMRI(MRIMixin, LinearPhysics):
 
     def _spec(self):
         m = self.mask
-        return self._mcache.get(m if m.dtype == torch.float32 else m.float(), m.shape[-2], m.shape[-1])
+        return self._mcache.get(m if m.dtype == torch.float32 else m.float(), self.three_d)
 
     def _maps(self) -> Tensor:
         cm = self.coil_maps
         return cm if cm.dtype == torch.complex64 else cm.to(torch.complex64)
 
+    def _check3d(self, t: Tensor, coil_dim: bool):
+        """shapes the 3-D kernels index by: volumes of the mask's (D,H,W) and mask / maps batches of 1 or B"""
+        dims = tuple(self.mask.shape[-3:])
+        ok = t.dim() == 5 + coil_dim and tuple(t.shape[-3:]) == dims and tuple(self.coil_maps.shape[-3:]) == dims
+        if not ok or (coil_dim and t.shape[2] != self.coil_maps.shape[1]):
+            raise ValueError(f"expected {'(B,2,N,D,H,W)' if coil_dim else '(B,2,D,H,W)'} with (D,H,W) = {dims} and "
+                             f"N = {self.coil_maps.shape[1]} coils, got {tuple(t.shape)}")
+        if self.mask.shape[0] not in (1, t.shape[0]):
+            raise ValueError(f"mask batch {self.mask.shape[0]} does not match input batch {t.shape[0]}")
+
     def _A_general(self, x):
         H, W = x.shape[-2:]
         cm = self._maps()
         N = cm.shape[1]
+        if self.three_d:
+            self._check3d(x, False)
+            return ops.spectral3d(x, *x.shape[-3:], fwd=True, inv=False, gmode=_ffi.G_MASK, mask=self._spec(), ncoil=N,
+                                  coil_mode=1, coil_maps=cm)
         if N > 1:
             return ops.spectral(x, H, W, fwd=True, inv=False, gmode=_ffi.G_MASK, mask=self._spec(), ncoil=N,
                                 coil_mode=1, coil_maps=cm)
@@ -471,6 +454,10 @@ class MultiCoilMRI(MRIMixin, LinearPhysics):
         H, W = y.shape[-2:]
         cm = self._maps()
         N = y.shape[2]
+        if self.three_d:
+            self._check3d(y, True)
+            return ops.spectral3d(y, *y.shape[-3:], fwd=False, inv=True, gmode=_ffi.G_MASK, mask=self._spec(), ncoil=N,
+                                  coil_mode=3 if rss else 2, coil_maps=cm)
         if N > 1:
             return ops.spectral(y, H, W, fwd=False, inv=True, gmode=_ffi.G_MASK, mask=self._spec(), ncoil=N,
                                 coil_mode=3 if rss else 2, coil_maps=cm)

@@ -116,6 +116,22 @@ int dinvk_spectral(const dinvk_spectral_args* args, void* workspace, size_t work
 /* build + cache the per-size tables now (call once before graph capture) */
 int dinvk_fft_prepare(int n, int centered);
 
+/* 3-D: the same operator with F the centred (or plain) orthonormal 3-D DFT of contiguous (D,H,W) volumes
+ * (deepinv/physics/mri.py:11-163 with three_d=True, MultiCoilMRI.A / A_adjoint on (B,2,N,D,H,W), mri.py:254-324).
+ * `args` means what it means for dinvk_spectral, with every "H,W" read as "D,H,W": B counts complex volumes, p0 / p1 / q0 /
+ * q1 / out are planar (B,2,D,H,W), and the mask is addressed as mask[b*mask_sb + ch*mask_sc + (d*H + h)*mask_sh + w]
+ * ((B,2,D,H,W) full mask: sb=2DHW sc=DHW sh=W).  Coils: coil_mode 0 uses no maps (see below); coil_mode 1..3 has the
+ * meaning above for any ncoil >= 1 (a single coil included), with x / out (batch,2,D,H,W), y (batch,2,ncoil,D,H,W), the
+ * rss volume (batch,1,D,H,W) and interleaved complex64 maps (batch|1, ncoil, D, H, W), coil_sb in complex elements.
+ * coil_mode 0 with ncoil = N > 1 transforms a plain stack of N volumes per sample: p0 / p1 / q0 / q1 / out are all
+ * (batch,2,N,D,H,W), no maps, and the mask is the sample's (b = volume / N), shared by its N volumes.
+ * Sizes as dinvk_spectral: each axis is a power-of-two or mixed radix 2/3/4/5/8/16 tile pass; an axis with another prime
+ * factor (or past the tile budget) takes an O(N^2) DFT, and the call then runs unfused (elementwise prologue / epilogue
+ * around the three axis transforms); D*H*W < 2^31.
+ * No launch for B == 0. */
+size_t dinvk_spectral3d_workspace_bytes(int B, int D, int H, int W);
+int dinvk_spectral3d(const dinvk_spectral_args* args, int D, void* workspace, size_t workspace_bytes, void* stream);
+
 /* Ramp filter of filtered back-projection (deepinv/physics/functional/radon.py:79-162): `rows` (>= 2)
  * signals of length N (contiguous, one per row — the angle-major sinogram memory (B*C*A, P)), each
  * zero-padded to L = max(64, 2^ceil(log2(2N))), multiplied by 2*rfft(f) with f the reference's spatial ramp
