@@ -80,6 +80,10 @@ _SIGNATURES = {
     "dinvk_conv_tc32_tail": (c_int, [c_void_p] * 5 + [c_int] * 6 + [c_void_p, c_void_p]),
     "dinvk_split16_to_nchw": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "dinvk_nchw_to_split16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "dinvk_conv3d_f32": (c_int, [c_void_p] * 6 + [c_int] * 8 + [c_void_p]),
+    "dinvk_conv3d_tc32": (c_int, [c_void_p] * 6 + [c_int] * 10 + [c_void_p, c_void_p]),
+    "dinvk_conv3d_tc32_head": (c_int, [c_void_p] * 4 + [c_int] * 6 + [c_float, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "dinvk_conv3d_tc32_tail": (c_int, [c_void_p] * 5 + [c_int] * 7 + [c_void_p, c_void_p]),
     "dinvk_tv_prox": (c_int, [c_void_p] * 6 + [c_int] * 5 + [c_float, C.c_double, C.c_double, c_int, c_int, c_int,
                                                                c_void_p, c_size_t, c_void_p]),
     "dinvk_tv_prox_workspace_bytes": (c_size_t, [c_int] * 4),

@@ -111,4 +111,11 @@ __host__ __device__ __forceinline__ float2 cconj(float2 a) { return make_float2(
 
 inline int ceil_div(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
 
+// true if the product of the (non-negative) factors stays below 2^62: element / byte offsets of the tensor fit int64
+inline bool product_fits(long long acc) { return acc >= 0; }
+template <class... T>
+inline bool product_fits(long long acc, long long f, T... rest) {
+  return acc >= 0 && f >= 0 && (f == 0 || acc <= (1LL << 62) / f) && product_fits(acc * f, rest...);
+}
+
 }  // namespace dinvk

@@ -262,6 +262,206 @@ __global__ void __launch_bounds__(256) conv2x2_f32_kernel(const float* __restric
 
 
 // ---------------------------------------------------------------------------------------------
+// 3-D (NCDHW) forward kernels for DRUNet(dim=3) (deepinv/models/drunet.py with Conv3d / ConvTranspose3d).
+//   3x3x3: the 2-D kernel's CTA (8 x 32 pixels of ONE depth plane x 32 output channels) walks the three input planes z - 1 ..
+//          z + 1 inside each 8-channel step; a plane outside the volume is the zero padding and is skipped.
+//   2x2x2 stride 2 and its transpose: the 2-D gather-GEMM-scatter with 8 taps.
+// Every offset is 64-bit: one 64-channel activation of a 64 x 256 x 256 volume is 2^28 elements.
+// ---------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256, 2) conv3x3x3_f32_kernel(const float* __restrict__ x, const float* __restrict__ xadd,
+                                                               const float* __restrict__ w, const float* __restrict__ bias,
+                                                               const float* __restrict__ res, float* __restrict__ out, int Cin,
+                                                               int Cout, int D, int H, int W, int tiles_x, int tiles, int act) {
+  __shared__ __align__(16) float s_in[C3_CC][C3_TH + 2][C3_ROWP];
+  __shared__ __align__(16) float s_w[C3_CC * 9][C3_WS];
+  const int tid = threadIdx.x;
+  const int tx = tid & 7, ty = (tid >> 3) & 7, tz = tid >> 6;
+  const long long plane = blockIdx.x / tiles;   // b * D + z
+  const int t = (int)(blockIdx.x - plane * tiles);
+  const int ty0 = (t / tiles_x) * C3_TH, tx0 = (t % tiles_x) * C3_TW;
+  const int co0 = blockIdx.y * C3_TC;
+  const long long b = plane / D;
+  const int z = (int)(plane - b * D);
+  const long long HW = (long long)H * W, DHW = HW * D;
+  const float* xb = x + b * Cin * DHW;
+  const float* ab = xadd ? xadd + b * Cin * DHW : nullptr;
+
+  float acc[4][8];
+#pragma unroll
+  for (int p = 0; p < 4; ++p)
+#pragma unroll
+    for (int q = 0; q < 8; ++q) acc[p][q] = 0.f;
+  float* s_in_flat = &s_in[0][0][0];
+  float* s_w_flat = &s_w[0][0];
+
+  for (int c0 = 0; c0 < Cin; c0 += C3_CC) {
+    for (int kz = 0; kz < 3; ++kz) {
+      const int zz = z + kz - 1;
+      if (zz < 0 || zz >= D) continue;   // CTA-uniform
+      for (int idx = tid; idx < C3_IN_ELEMS; idx += 256) {
+        const int c = idx / ((C3_TH + 2) * (C3_TW + 2));
+        const int rem = idx - c * ((C3_TH + 2) * (C3_TW + 2));
+        const int r = rem / (C3_TW + 2), col = rem - r * (C3_TW + 2);
+        const int gy = ty0 + r - 1, gx = tx0 + col - 1;
+        float v = 0.f;
+        if (c0 + c < Cin && gy >= 0 && gy < H && gx >= 0 && gx < W) {
+          const long long o = (long long)(c0 + c) * DHW + (long long)zz * HW + (long long)gy * W + gx;
+          v = __ldg(xb + o);
+          if (ab) v += __ldg(ab + o);
+        }
+        s_in_flat[idx + 2 * (idx / (C3_TW + 2))] = v;
+      }
+      // w[(co, ci, kz, ky, kx)] -> s_w[(ci, ky * 3 + kx)][co], the 2-D kernel's staging order
+      for (int idx = tid; idx < C3_CC * 9 * C3_TC; idx += 256) {
+        const int blk = idx >> 5;
+        const int ck = (blk % 9) * 8 + (idx & 7), co = (blk / 9) * 4 + ((idx >> 3) & 3);
+        const int ci = ck / 9, tap = ck - ci * 9;
+        float v = 0.f;
+        if (c0 + ci < Cin && co0 + co < Cout) v = __ldg(w + (((long long)(co0 + co) * Cin + c0 + ci) * 3 + kz) * 9 + tap);
+        s_w_flat[ck * C3_WS + co] = v;
+      }
+      __syncthreads();
+#pragma unroll
+      for (int c = 0; c < C3_CC; ++c) {
+#pragma unroll
+        for (int ky = 0; ky < 3; ++ky) {
+          const float4 i0 = *reinterpret_cast<const float4*>(&s_in[c][ty + ky][tx * 4]);
+          const float2 i1 = *reinterpret_cast<const float2*>(&s_in[c][ty + ky][tx * 4 + 4]);
+          const float in6[6] = {i0.x, i0.y, i0.z, i0.w, i1.x, i1.y};
+#pragma unroll
+          for (int kx = 0; kx < 3; ++kx) {
+            const float4 w0 = *reinterpret_cast<const float4*>(&s_w[c * 9 + ky * 3 + kx][tz * 8]);
+            const float4 w1 = *reinterpret_cast<const float4*>(&s_w[c * 9 + ky * 3 + kx][tz * 8 + 4]);
+            const float wv[8] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
+#pragma unroll
+            for (int p = 0; p < 4; ++p)
+#pragma unroll
+              for (int q = 0; q < 8; ++q) acc[p][q] = fmaf(in6[p + kx], wv[q], acc[p][q]);
+          }
+        }
+      }
+      __syncthreads();
+    }
+  }
+
+  const int gy = ty0 + ty;
+  if (gy < H) {
+#pragma unroll
+    for (int q = 0; q < 8; ++q) {
+      const int co = co0 + tz * 8 + q;
+      if (co < Cout) {
+        const float bv = bias ? __ldg(bias + co) : 0.f;
+        const long long ob = ((b * Cout + co) * D + z) * HW + (long long)gy * W;
+#pragma unroll
+        for (int p = 0; p < 4; ++p) {
+          const int gx = tx0 + tx * 4 + p;
+          if (gx < W) {
+            float v = acc[p][q] + bv;
+            if (act == 1) v = fmaxf(v, 0.f);
+            if (res) v += __ldg(res + ob + gx);
+            out[ob + gx] = v;
+          }
+        }
+      }
+    }
+  }
+}
+
+// gather-GEMM-scatter for the 2x2x2 stride-2 conv (mode 1) and its transpose (mode 2), tap = dz * 4 + dy * 2 + dx
+//   mode 1: M = B*Do*Ho*Wo, N = Cout, K = 8*Cin;  A(m,k) = (x+xadd)[b, k/8, 2zo+dz, 2yo+dy, 2xo+dx],  Wt(k,n) = w[n*K + k]
+//   mode 2: M = B*D*H*W,    N = 8*Cout, K = Cin;  A(m,k) = (x+xadd)[b, k, z, y, x],  Wt(k,n) = w[k*N + n],
+//           out[b, n/8, 2z+dz, 2y+dy, 2x+dx]
+__global__ void __launch_bounds__(256) conv2x2x2_f32_kernel(const float* __restrict__ x, const float* __restrict__ xadd,
+                                                            const float* __restrict__ w, const float* __restrict__ bias,
+                                                            const float* __restrict__ res, float* __restrict__ out,
+                                                            int B, int Cin, int Cout, int D, int H, int W, int mode, int act) {
+  __shared__ float sA[G_TK][G_TM + 1];
+  __shared__ float sW[G_TK][G_TN + 1];
+  const int tid = threadIdx.x;
+  const int Do = D / 2, Ho = H / 2, Wo = W / 2;
+  const long long HW = (long long)H * W, DHW = HW * D, OV = (long long)Do * Ho * Wo;
+  const long long M = mode == 1 ? (long long)B * OV : (long long)B * DHW;
+  const int N = mode == 1 ? Cout : 8 * Cout;
+  const int K = mode == 1 ? 8 * Cin : Cin;
+  const long long m0 = (long long)blockIdx.x * G_TM;
+  const int n0 = blockIdx.y * G_TN;
+  const int tm = tid & 31, tn = tid >> 5;
+  float acc[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
+
+  for (int k0 = 0; k0 < K; k0 += G_TK) {
+    for (int idx = tid; idx < G_TK * G_TM; idx += 256) {
+      const int kk = idx / G_TM, mm = idx - kk * G_TM;
+      const long long m = m0 + mm;
+      const int k = k0 + kk;
+      float v = 0.f;
+      if (m < M && k < K) {
+        long long o;
+        if (mode == 1) {
+          const long long bb = m / OV, p = m - bb * OV;
+          const int xo = (int)(p % Wo), yo = (int)((p / Wo) % Ho), zo = (int)(p / ((long long)Wo * Ho));
+          const int c = k >> 3, dz = (k >> 2) & 1, dy = (k >> 1) & 1, dx = k & 1;
+          o = (bb * Cin + c) * DHW + (long long)(2 * zo + dz) * HW + (long long)(2 * yo + dy) * W + (2 * xo + dx);
+        } else {
+          const long long bb = m / DHW, p = m - bb * DHW;
+          o = (bb * Cin + k) * DHW + p;
+        }
+        v = __ldg(x + o);
+        if (xadd) v += __ldg(xadd + o);
+      }
+      sA[kk][mm] = v;
+    }
+    for (int idx = tid; idx < G_TK * G_TN; idx += 256) {
+      int kk, nn;
+      if (mode == 1) { nn = idx / G_TK; kk = idx - nn * G_TK; }
+      else { kk = idx / G_TN; nn = idx - kk * G_TN; }
+      const int k = k0 + kk, n = n0 + nn;
+      float v = 0.f;
+      if (k < K && n < N) v = mode == 1 ? __ldg(w + (long long)n * K + k) : __ldg(w + (long long)k * N + n);
+      sW[kk][nn] = v;
+    }
+    __syncthreads();
+#pragma unroll 8
+    for (int kk = 0; kk < G_TK; ++kk) {
+      const float a0 = sA[kk][tm], a1 = sA[kk][tm + 32];
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const float wv = sW[kk][tn * 4 + q];
+        acc[0][q] = fmaf(a0, wv, acc[0][q]);
+        acc[1][q] = fmaf(a1, wv, acc[1][q]);
+      }
+    }
+    __syncthreads();
+  }
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const long long m = m0 + tm + 32 * i;
+    if (m >= M) continue;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const int n = n0 + tn * 4 + q;
+      if (n >= N) continue;
+      long long o;
+      int co;
+      if (mode == 1) {
+        const long long bb = m / OV, p = m - bb * OV;
+        co = n;
+        o = (bb * Cout + co) * OV + p;
+      } else {
+        const long long bb = m / DHW, p = m - bb * DHW;
+        const int z = (int)(p / HW), y = (int)((p - z * HW) / W), xx = (int)(p - z * HW - (long long)y * W);
+        co = n >> 3;
+        const int dz = (n >> 2) & 1, dy = (n >> 1) & 1, dx = n & 1;
+        o = (bb * Cout + co) * (8 * DHW) + (long long)(2 * z + dz) * (4 * HW) + (long long)(2 * y + dy) * (2 * W) + (2 * xx + dx);
+      }
+      float v = acc[i][q] + (bias ? __ldg(bias + co) : 0.f);
+      if (act == 1) v = fmaxf(v, 0.f);
+      if (res) v += __ldg(res + o);
+      out[o] = v;
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
 // Backward kernels of the fp32 path (training through the denoiser: unfolded / DEQ models,
 // deepinv/unfolded/unfolded.py:9-120, deep_equilibrium.py:70-139 — SURVEY §8(f) item 2).
 // Data gradients reuse the forward kernels (a 3x3 convolution with the transposed, flipped filter;
@@ -530,6 +730,33 @@ extern "C" int dinvk_conv_f32(const float* x, const float* xadd, const float* we
     const int N = kind == 1 ? Cout : 4 * Cout;
     DINVK_LAUNCH(conv2x2_f32_kernel, dim3((unsigned)ceil_div(M, G_TM), ceil_div(N, G_TN)), dim3(256), 0, stream, x, xadd,
                  weight, bias, res, out, B, Cin, Cout, H, W, kind, act);
+  }
+  return DINVK_POST_LAUNCH();
+}
+
+extern "C" int dinvk_conv3d_f32(const float* x, const float* xadd, const float* weight, const float* bias, const float* res,
+                                float* out, int B, int Cin, int Cout, int D, int H, int W, int kind, int act, void* stream) {
+  DINVK_CHECK_ARG(x && weight && out, "dinvk_conv3d_f32: null pointer");
+  DINVK_CHECK_ARG(B >= 0 && Cin >= 1 && Cout >= 1 && D >= 1 && H >= 1 && W >= 1, "dinvk_conv3d_f32: bad shape");
+  DINVK_CHECK_ARG(kind >= 0 && kind <= 2, "dinvk_conv3d_f32: kind %d not in 0..2", kind);
+  DINVK_CHECK_ARG(act == 0 || act == 1, "dinvk_conv3d_f32: act %d", act);
+  DINVK_CHECK_ARG(kind != 1 || (D % 2 == 0 && H % 2 == 0 && W % 2 == 0), "dinvk_conv3d_f32: strided conv needs even D, H, W (got %d, %d, %d)",
+                  D, H, W);
+  // the transposed conv's output is the largest tensor of a call: 8 voxels per input voxel
+  DINVK_CHECK_ARG(product_fits(B, Cin > Cout ? Cin : Cout, D, H, W, 8, 4), "dinvk_conv3d_f32: volume (%d, %d, %d, %d, %d) too large", B,
+                  Cin > Cout ? Cin : Cout, D, H, W);
+  if (B == 0) return DINVK_OK;
+  if (kind == 0) {
+    const int tiles_x = ceil_div(W, C3_TW), tiles = tiles_x * ceil_div(H, C3_TH);
+    DINVK_CHECK_ARG((long long)tiles * D * B < (1LL << 31) && ceil_div(Cout, C3_TC) <= 65535, "dinvk_conv3d_f32: grid too large");
+    DINVK_LAUNCH(conv3x3x3_f32_kernel, dim3((unsigned)((long long)tiles * D * B), ceil_div(Cout, C3_TC)), dim3(256), 0, stream, x, xadd,
+                 weight, bias, res, out, Cin, Cout, D, H, W, tiles_x, tiles, act);
+  } else {
+    const long long M = kind == 1 ? (long long)B * (D / 2) * (H / 2) * (W / 2) : (long long)B * D * H * W;
+    const int N = kind == 1 ? Cout : 8 * Cout;
+    DINVK_CHECK_ARG((M + G_TM - 1) / G_TM < (1LL << 31) && ceil_div(N, G_TN) <= 65535, "dinvk_conv3d_f32: grid too large");
+    DINVK_LAUNCH(conv2x2x2_f32_kernel, dim3((unsigned)((M + G_TM - 1) / G_TM), ceil_div(N, G_TN)), dim3(256), 0, stream, x, xadd,
+                 weight, bias, res, out, B, Cin, Cout, D, H, W, kind, act);
   }
   return DINVK_POST_LAUNCH();
 }

@@ -40,6 +40,7 @@ inline void stg256(void* p, const uint32_t (&r)[8]) { std::memcpy(p, r, 32); }
 #include <algorithm>
 #include <cstdlib>
 #include <cstring>
+#include <type_traits>
 
 namespace dinvk {
 namespace t32 {
@@ -139,10 +140,13 @@ __device__ __forceinline__ void release_stage(uint64_t* bar) {
   if ((threadIdx.x & 31) == 0) tc::mbar_arrive(bar);
 }
 
-struct Maps {
-  CUtensorMap a[4];  // activation views: one (3x3, up) or one per tap (2x2 stride-2 down)
+template <int NA>
+struct MapsT {
+  CUtensorMap a[NA];  // activation views: one (3x3, up) or one per tap (2x2 stride-2 down: 4 taps in 2-D, 8 in 3-D)
   CUtensorMap b;
 };
+using Maps = MapsT<4>;
+using Maps3 = MapsT<8>;
 
 struct Params {
   int B, H, W, Cin, Cout;   // H, W: the pixel grid the GEMM rows tile (3x3: image; down: OUTPUT grid; up: INPUT grid)
@@ -161,6 +165,11 @@ struct Params {
                             // the CTAs that share its activations run at the same time and all but the first read them from L2
                             // (1 = all pixel tiles of N tile 0 first: every activation byte crosses HBM n_tiles times); divides n_tiles
 };
+struct Params3 : Params {
+  int D;                    // depth of the grid the GEMM rows tile; B counts the B * D depth planes
+};
+__device__ __forceinline__ int depth_of(const Params3& p) { return p.D; }
+__device__ __forceinline__ int depth_of(const Params&) { return 1; }
 
 // work item t -> (pixel tile, N tile): t = ((nt / g) * pixel_tiles + pt) * g + nt % g, g = P.ngrp
 __device__ __forceinline__ void tile_index(const Params& P, int pixel_tiles, int t, int& pt, int& nt) {
@@ -421,8 +430,12 @@ __device__ __forceinline__ void epilogue_t(const Params& P, const float* v, floa
   if (bad && P.flag) atomicOr(P.flag, 1);
 }
 
-template <class F>
-__global__ void __launch_bounds__(THREADS, 1) conv_tc32_kernel(const __grid_constant__ Maps M, const Params P) {
+// D3 = true: the same kernel on NDHWC volumes.  The activation maps are rank 5 (words, W, H, D, B), a work item is a 16 x 8
+// pixel tile of one depth plane (P.B = B * D planes), and the taps are the 27 (dz, dy, dx) of a 3x3x3 convolution (k =
+// ((kz * 3 + ky) * 3 + kx) * Cin + c), the 8 maps of a 2x2x2 stride-2 convolution, or the single map of its transpose, whose
+// N tile names the output sub-voxel tap = dz * 4 + dy * 2 + dx.  TMA's zero fill outside W, H and D is the zero padding.
+template <class F, bool D3>
+__global__ void __launch_bounds__(THREADS, 1) conv_tc32_kernel(const __grid_constant__ MapsT<D3 ? 8 : 4> M, const std::conditional_t<D3, Params3, Params> P) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
   __shared__ __align__(8) uint64_t full_bar[STAGES];
@@ -455,8 +468,17 @@ __global__ void __launch_bounds__(THREADS, 1) conv_tc32_kernel(const __grid_cons
           uint8_t* sa = smem + s * STAGE;
           tc::mbar_arrive_expect_tx(&full_bar[s], STAGE);
           // channel blocks 2kc and 2kc+1: one 128-byte row ([hi CH | lo CH]) each, at element offset 2 CH * block
-          tc::tma_load_4d(sa, &M.a[P.amap[tap]], &full_bar[s], (2 * kc) * (2 * F::CH), x0 + P.dx[tap], y0 + P.dy[tap], b);
-          tc::tma_load_4d(sa + A_TILE, &M.a[P.amap[tap]], &full_bar[s], (2 * kc + 1) * (2 * F::CH), x0 + P.dx[tap], y0 + P.dy[tap], b);
+          if constexpr (D3) {
+            const int bb = b / depth_of(P), z = b - bb * depth_of(P);
+            const bool k27 = P.ntaps == 27;
+            const int m = k27 ? 0 : tap;   // 2x2x2 down: one map per tap; transposed: the single map
+            const int dz = k27 ? tap / 9 - 1 : 0, dy = k27 ? (tap / 3) % 3 - 1 : 0, dx = k27 ? tap % 3 - 1 : 0;
+            tc::tma_load_5d(sa, &M.a[m], &full_bar[s], (2 * kc) * (2 * F::CH), x0 + dx, y0 + dy, z + dz, bb);
+            tc::tma_load_5d(sa + A_TILE, &M.a[m], &full_bar[s], (2 * kc + 1) * (2 * F::CH), x0 + dx, y0 + dy, z + dz, bb);
+          } else {
+            tc::tma_load_4d(sa, &M.a[P.amap[tap]], &full_bar[s], (2 * kc) * (2 * F::CH), x0 + P.dx[tap], y0 + P.dy[tap], b);
+            tc::tma_load_4d(sa + A_TILE, &M.a[P.amap[tap]], &full_bar[s], (2 * kc + 1) * (2 * F::CH), x0 + P.dx[tap], y0 + P.dy[tap], b);
+          }
           tc::tma_load_2d(sa + 2 * A_TILE, &M.b, &full_bar[s], tap * P.Cin + kc * (2 * F::CH), nt * 128);
           if (++s == STAGES) { s = 0; ph ^= 1; }
         }
@@ -507,7 +529,19 @@ __global__ void __launch_bounds__(THREADS, 1) conv_tc32_kernel(const __grid_cons
         if (P.mode == 2) return ((long long)b * (2 * P.H) + 2 * y + (tap >> 1)) * (2LL * P.W) + 2 * x + (tap & 1);
         return ((long long)b * P.H + y) * P.W + x;
       };
-      epilogue<F>(P, v, reinterpret_cast<float*>(smem + STAGES * STAGE) + warp * STG_WARP, pixel_of, nt * 64 - tap * P.Cout);
+      // 3-D: b is the plane bb * D + z, so that the same-grid offset above is the NDHWC one; the up-scatter adds dz = tap >> 2
+      const auto pixel_of3 = [&](int m) -> long long {
+        const int mm = 64 * wg + 16 * (warp & 3) + m;
+        const int y = y0 + mm / TX, x = x0 + mm % TX;
+        if (!(y < P.H && x < P.W)) return -1;
+        if (P.mode != 2) return ((long long)b * P.H + y) * P.W + x;
+        const int D = depth_of(P), bb = b / D, z = b - bb * D;
+        return (((long long)bb * (2 * D) + 2 * z + (tap >> 2)) * (2 * P.H) + 2 * y + ((tap >> 1) & 1)) * (2LL * P.W) + 2 * x + (tap & 1);
+      };
+      if constexpr (D3)
+        epilogue<F>(P, v, reinterpret_cast<float*>(smem + STAGES * STAGE) + warp * STG_WARP, pixel_of3, nt * 64 - tap * P.Cout);
+      else
+        epilogue<F>(P, v, reinterpret_cast<float*>(smem + STAGES * STAGE) + warp * STG_WARP, pixel_of, nt * 64 - tap * P.Cout);
     }
   }
 }
@@ -683,6 +717,7 @@ struct HeadParams {
   float fill_scalar; const float* fill_batch; int has_fill; int relu;
   int* flag;
 };
+struct Head3Params : HeadParams { int D; };   // + depth of the NCDHW volume
 
 template <class F, int CT>
 __global__ void __launch_bounds__(256) head_tc32_kernel(const HeadParams P) {
@@ -854,6 +889,7 @@ struct TailParams {
   int B, H, W, C, Cout;
   const int* flag;   // overflow flag of the network (FmtF16): set -> the output is NaN
 };
+struct Tail3Params : TailParams { int D; };   // + depth of the volume
 constexpr int TL_TX = 32, TL_TY = 8;
 
 template <class F, int CO>
@@ -1093,6 +1129,164 @@ __global__ void __launch_bounds__(256) tail64_tc32_kernel(const TailParams P) {
 #undef TL_ROW
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// 3-D HEAD and TAIL (CUDA cores) for DRUNet(dim=3).
+// head3d: 3x3x3 convolution from the NCDHW fp32 volume (+ the constant noise-level channel) to Cout split channels of the
+//   NDHWC layout; the thread-per-pixel head with 27 taps: one thread per voxel, its 27 * CT inputs in registers, the weights
+//   of 64 output channels at a time in shared memory, read as 128-bit broadcasts.
+// tail3d: 3x3x3 convolution from C split channels to Cout <= 4 fp32 NCDHW channels (+ bias, + NCDHW addend).  A CTA owns a
+//   32 x 8-pixel tile of one output plane and stages, per input plane z - 1 .. z + 1 and per chunk of <= 64 channels, the
+//   (32 + 2) x (8 + 2) halo tile as hi + lo in shared memory ([position][chunk + 4] words, as tail_tc32_kernel).
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int HD3_CO = 64;   // output channels per weight stage of the 3-D head
+
+template <class F, int CT>
+__global__ void __launch_bounds__(256) head3d_tc32_kernel(const Head3Params P) {
+  constexpr int KR = 27 * CT, KP = (KR + 3) & ~3;
+  __shared__ __align__(16) float sw[HD3_CO * KP];   // (Cout, CT, 3, 3, 3) -> sw[(co - co0) * KP + c * 27 + tap], zero padded
+  const long long HW = (long long)P.H * P.W, DHW = HW * P.D;
+  const long long npix = (long long)P.B * DHW;
+  const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const bool live = p < npix;   // every thread stays for the weight stages
+  const long long b = live ? p / DHW : 0, rem = live ? p - b * DHW : 0;
+  const int z = (int)(rem / HW), rem2 = (int)(rem - z * HW);
+  const int y = rem2 / P.W, x = rem2 - y * P.W;
+  const float fillv = P.has_fill ? (P.fill_batch ? __ldg(P.fill_batch + b) : P.fill_scalar) : 0.f;
+  float in[KP];
+#pragma unroll
+  for (int k = KR; k < KP; ++k) in[k] = 0.f;
+  const float* img = P.x + b * P.C * DHW;
+#pragma unroll
+  for (int c = 0; c < CT; ++c) {
+#pragma unroll
+    for (int tap = 0; tap < 27; ++tap) {
+      const int zz = z + tap / 9 - 1, yy = y + (tap / 3) % 3 - 1, xx = x + tap % 3 - 1;
+      const bool inb = live && zz >= 0 && zz < P.D && yy >= 0 && yy < P.H && xx >= 0 && xx < P.W;
+      float val = 0.f;
+      if (inb) val = (c < P.C) ? __ldg(img + (long long)c * DHW + (long long)zz * HW + (long long)yy * P.W + xx) : fillv;
+      in[c * 27 + tap] = val;
+    }
+  }
+  typename F::elem* o = static_cast<typename F::elem*>(P.out) + p * P.Cout * 2;
+  bool bad = false;
+  for (int co0 = 0; co0 < P.Cout; co0 += HD3_CO) {
+    const int nco = min(HD3_CO, P.Cout - co0);
+    __syncthreads();
+    for (int i = threadIdx.x; i < nco * KP; i += blockDim.x) {
+      const int co = i / KP, k = i - co * KP;
+      sw[i] = k < KR ? __ldg(P.w + (long long)(co0 + co) * KR + k) : 0.f;
+    }
+    __syncthreads();
+    if (!live) continue;
+    for (int c1 = 0; c1 < nco; c1 += F::CH) {
+      float v[F::CH];
+#pragma unroll
+      for (int i = 0; i < F::CH; ++i) {
+        float a = P.bias ? __ldg(P.bias + co0 + c1 + i) : 0.f;
+        const float4* wr = reinterpret_cast<const float4*>(sw + (c1 + i) * KP);
+#pragma unroll
+        for (int k = 0; k < KP / 4; ++k) {
+          const float4 w4 = wr[k];
+          a = fmaf(in[4 * k], w4.x, a); a = fmaf(in[4 * k + 1], w4.y, a);
+          a = fmaf(in[4 * k + 2], w4.z, a); a = fmaf(in[4 * k + 3], w4.w, a);
+        }
+        v[i] = P.relu ? fmaxf(a, 0.f) : a;
+      }
+      bad |= store_split<F>(o + (co0 + c1) * 2, v);
+    }
+  }
+  if (bad && P.flag) atomicOr(P.flag, 1);
+}
+
+constexpr int TL3_CC = 64;   // channels per staged chunk of the 3-D tail
+
+template <class F, int CO>
+__global__ void __launch_bounds__(256) tail3d_tc32_kernel(const Tail3Params P) {
+#ifndef DINVK_EMUL
+  extern __shared__ __align__(16) float sm[];
+#else
+  float* sm = reinterpret_cast<float*>(::emul::dyn_smem());
+#endif
+  const int C = P.C, CP = TL3_CC + 4;
+  float* sx = sm;                                    // (TL_TY+2)*(TL_TX+2) positions x CP
+  float* swt = sm + (TL_TY + 2) * (TL_TX + 2) * CP;  // [co][tap 27][C]
+  const int tiles_x = (P.W + TL_TX - 1) / TL_TX, tiles = tiles_x * ((P.H + TL_TY - 1) / TL_TY);
+  const long long plane = blockIdx.x / tiles;        // b * D + z
+  const int r = (int)(blockIdx.x - plane * tiles);
+  const long long b = plane / P.D;
+  const int z = (int)(plane - b * P.D);
+  const int y0 = (r / tiles_x) * TL_TY, x0 = (r % tiles_x) * TL_TX;
+  for (int i = threadIdx.x; i < CO * 27 * C; i += blockDim.x) {   // (Cout, C, 3, 3, 3) -> [co][tap][c]; rows co >= Cout are zero
+    const int co = i / (27 * C), rem = i - co * 27 * C, tap = rem / C, c = rem - tap * C;
+    swt[i] = co < P.Cout ? __ldg(P.w + ((long long)co * C + c) * 27 + tap) : 0.f;
+  }
+  const int ty = threadIdx.x / TL_TX, tx = threadIdx.x % TL_TX;
+  const int y = y0 + ty, x = x0 + tx;
+  float acc[CO];
+#pragma unroll
+  for (int co = 0; co < CO; ++co) acc[co] = 0.f;
+  const int npos = (TL_TY + 2) * (TL_TX + 2);
+  for (int c0 = 0; c0 < C; c0 += TL3_CC) {
+    const int cc = min(TL3_CC, C - c0), q4 = cc / 4;
+    for (int kz = 0; kz < 3; ++kz) {
+      const int zz = z + kz - 1;
+      if (zz < 0 || zz >= P.D) continue;   // CTA-uniform: the plane is the zero padding
+      __syncthreads();                     // the previous plane's reads are done (and the weights are staged)
+      for (int i = threadIdx.x; i < npos * q4; i += blockDim.x) {
+        const int pos = i / q4, cq = i - pos * q4;
+        const int yy = y0 + pos / (TL_TX + 2) - 1, xx = x0 + pos % (TL_TX + 2) - 1;
+        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (yy >= 0 && yy < P.H && xx >= 0 && xx < P.W) {
+          const int c = c0 + cq * 4, blk = c / F::CH, ib = c % F::CH;
+          const typename F::elem* src = static_cast<const typename F::elem*>(P.x) +
+                                        (((b * P.D + zz) * P.H + yy) * P.W + xx) * C * 2 + blk * 2 * F::CH + ib;
+          if constexpr (F::ID == 0) {
+            const float4 h = __ldg(reinterpret_cast<const float4*>(src));
+            const float4 l = __ldg(reinterpret_cast<const float4*>(src + F::CH));
+            v = make_float4(h.x + l.x, h.y + l.y, h.z + l.z, h.w + l.w);
+          } else {
+            const uint2 hu = __ldg(reinterpret_cast<const uint2*>(src)), lu = __ldg(reinterpret_cast<const uint2*>(src + F::CH));
+            const float2 h0 = __half22float2(*reinterpret_cast<const __half2*>(&hu.x)), h1 = __half22float2(*reinterpret_cast<const __half2*>(&hu.y));
+            const float2 l0 = __half22float2(*reinterpret_cast<const __half2*>(&lu.x)), l1 = __half22float2(*reinterpret_cast<const __half2*>(&lu.y));
+            v = make_float4(h0.x + l0.x * F::CORR, h0.y + l0.y * F::CORR, h1.x + l1.x * F::CORR, h1.y + l1.y * F::CORR);
+          }
+        }
+        *reinterpret_cast<float4*>(sx + pos * CP + cq * 4) = v;
+      }
+      __syncthreads();
+#pragma unroll 1
+      for (int tap = 0; tap < 9; ++tap) {
+        const float* px = sx + ((ty + tap / 3) * (TL_TX + 2) + tx + tap % 3) * CP;
+        const float* wt = swt + (kz * 9 + tap) * C + c0;
+#pragma unroll 4
+        for (int c = 0; c < cc; c += 4) {
+          const float4 a = *reinterpret_cast<const float4*>(px + c);
+#pragma unroll
+          for (int co = 0; co < CO; ++co) {
+            const float4 w4 = *reinterpret_cast<const float4*>(wt + co * 27 * C + c);
+            acc[co] = fmaf(a.x, w4.x, acc[co]); acc[co] = fmaf(a.y, w4.y, acc[co]);
+            acc[co] = fmaf(a.z, w4.z, acc[co]); acc[co] = fmaf(a.w, w4.w, acc[co]);
+          }
+        }
+      }
+    }
+  }
+  const bool poisoned = P.flag && *reinterpret_cast<const volatile int*>(P.flag) != 0;
+  if (y < P.H && x < P.W) {
+    const long long HW = (long long)P.H * P.W;
+#pragma unroll
+    for (int co = 0; co < CO; ++co) {
+      if (co < P.Cout) {
+        const long long o = ((b * P.Cout + co) * P.D + z) * HW + (long long)y * P.W + x;
+        float val = acc[co] + (P.bias ? __ldg(P.bias + co) : 0.f);
+        if (P.add) val += __ldg(P.add + o);
+        if (poisoned) val = __uint_as_float(0x7fc00000u);
+        P.out[o] = val;
+      }
+    }
+  }
+}
+
 // split layout -> NCHW fp32 (tests / debugging): out[b,c,y,x] = hi + lo
 template <class F>
 __global__ void __launch_bounds__(256) split_to_nchw_kernel(const typename F::elem* __restrict__ in, float* __restrict__ out, int C, int H, int W,
@@ -1213,7 +1407,71 @@ static int conv_generic(const void* x, const void* weight, const float* bias, co
   // every 2x2 layer gains from sharing the activation tile between its N tiles (down 64 -> 128: 402 -> 297 us, up 256 -> 128: 415 -> 263 us):
   // with the N tile outermost each activation byte crossed HBM n_tiles (2 .. 8) times
   P.ngrp = getenv("DINVK_TC32_NT_OUTER") ? 1 : P.n_tiles;
-  return launch_persistent(conv_tc32_kernel<F>, THREADS, SMEM, (long long)P.B * P.tiles_y * P.tiles_x * P.n_tiles, stream, M, P);
+  return launch_persistent(conv_tc32_kernel<F, false>, THREADS, SMEM, (long long)P.B * P.tiles_y * P.tiles_x * P.n_tiles, stream, M, P);
+}
+
+// the 3-D per-tap convolutions on NDHWC split volumes (B, D, H, W, C/CH, 2, CH):
+// kind 0: 3x3x3 stride 1 zero-pad 1 (K = 27*Cin, k = ((kz*3+ky)*3+kx)*Cin + c)
+// kind 1: 2x2x2 stride 2 (K = 8*Cin, k = (dz*4+dy*2+dx)*Cin + c), out (B, D/2, H/2, W/2, Cout)
+// kind 2: transposed 2x2x2 stride 2 (K = Cin, GEMM column = (dz*4+dy*2+dx)*Cout + co), out (B, 2D, 2H, 2W, Cout)
+template <class F>
+static int conv_generic3d(const void* x, const void* weight, const float* bias, const void* res, const void* res2, void* out, int B, int D,
+                          int H, int W, int Cin, int Cout, int kind, int act, int window, int* flag, void* stream) {
+  DINVK_CHECK_ARG(x && weight && out, "conv3d_tc32: null pointer");
+  DINVK_CHECK_ARG(B >= 0 && D >= 1 && H >= 1 && W >= 1, "conv3d_tc32: bad shape");
+  DINVK_CHECK_ARG(kind >= 0 && kind <= 2, "conv3d_tc32: kind=%d not in 0..2", kind);
+  DINVK_CHECK_ARG(Cin % (2 * F::CH) == 0 && Cin >= 2 * F::CH, "conv3d_tc32: Cin=%d must be a multiple of %d", Cin, 2 * F::CH);
+  DINVK_CHECK_ARG(Cout % 64 == 0 && Cout >= 64, "conv3d_tc32: Cout=%d must be a multiple of 64", Cout);
+  DINVK_CHECK_ARG(kind != 1 || (D % 2 == 0 && H % 2 == 0 && W % 2 == 0), "conv3d_tc32: 2x2x2 stride-2 needs even D, H, W (got %d, %d, %d)",
+                  D, H, W);
+  DINVK_CHECK_ARG(kind == 0 || (!res && !res2), "conv3d_tc32: residual inputs are for kind 0 only");
+  DINVK_CHECK_ARG(epilogue_aligned(bias, res, res2, out), "conv3d_tc32: bias, res, res2 and out must be 16-byte aligned");
+  // element offsets of the largest tensor (the transposed conv's output: 8 voxels per input voxel, 2 words per channel)
+  DINVK_CHECK_ARG(product_fits(B, D, H, W, 8, 2 * F::EB, std::max(Cin, Cout)), "conv3d_tc32: volume (%d, %d, %d, %d) x %d channels too large",
+                  B, D, H, W, std::max(Cin, Cout));
+  if (B == 0) return DINVK_OK;
+  Maps3 M;
+  Params3 P{};
+  int rc;
+  const uint64_t px = (uint64_t)Cin * 2 * F::EB;  // bytes per input voxel
+  P.Cin = Cin; P.Cout = Cout;
+  P.kc_per_tap = Cin / (2 * F::CH);
+  P.relu = act; P.res = res; P.res2 = res2; P.out = out; P.bias = bias; P.flag = flag;
+  P.win = window > 0 ? window : default_window();
+  const uint32_t abox[5] = {2 * F::CH, TX, TY, 1, 1};
+  long long K = Cin, rows = 2LL * Cout;
+  const uint64_t plane = px * W * H, vol = plane * D;
+  if (kind == 1) {
+    const uint64_t adims[5] = {(uint64_t)Cin * 2, (uint64_t)(W / 2), (uint64_t)(H / 2), (uint64_t)(D / 2), (uint64_t)B};
+    const uint64_t astrides[4] = {2 * px, 2 * px * W, 2 * plane, vol};
+    for (int t = 0; t < 8; ++t) {
+      const char* base = reinterpret_cast<const char*>(x) + (((long long)(t >> 2) * H + ((t >> 1) & 1)) * W + (t & 1)) * px;
+      if ((rc = map_split<F>(&M.a[t], base, 5, adims, astrides, abox, "tc32 3-D activations"))) return rc;
+    }
+    K = 8LL * Cin;
+    P.D = D / 2; P.H = H / 2; P.W = W / 2; P.ntaps = 8; P.n_tiles = Cout / 64;
+  } else {
+    const uint64_t adims[5] = {(uint64_t)Cin * 2, (uint64_t)W, (uint64_t)H, (uint64_t)D, (uint64_t)B}, astrides[4] = {px, px * W, plane, vol};
+    if ((rc = map_split<F>(&M.a[0], x, 5, adims, astrides, abox, "tc32 3-D activations"))) return rc;
+    for (int t = 1; t < 8; ++t) M.a[t] = M.a[0];
+    P.D = D; P.H = H; P.W = W;
+    if (kind == 0) {
+      K = 27LL * Cin;
+      P.ntaps = 27; P.n_tiles = Cout / 64;
+    } else {
+      rows = 16LL * Cout;
+      P.ntaps = 1; P.mode = 2; P.n_tiles = 8 * Cout / 64;
+    }
+  }
+  const uint64_t wdims[2] = {(uint64_t)K, (uint64_t)rows}, wstride = (uint64_t)K * F::EB;
+  const uint32_t wbox[2] = {2 * F::CH, 128};
+  if ((rc = map_split<F>(&M.b, weight, 2, wdims, &wstride, wbox, "tc32 3-D weights"))) return rc;
+  P.tiles_x = ceil_div(P.W, TX); P.tiles_y = ceil_div(P.H, TY);
+  const long long items = (long long)B * P.D * P.tiles_y * P.tiles_x * P.n_tiles;
+  DINVK_CHECK_ARG(items < (1LL << 31), "conv3d_tc32: %lld work items exceed the kernel's 32-bit tile index", items);
+  P.B = B * P.D;   // the kernel's work items walk the depth planes of every volume
+  P.ngrp = P.n_tiles;
+  return launch_persistent(conv_tc32_kernel<F, true>, THREADS, SMEM, items, stream, M, P);
 }
 
 template <class F>
@@ -1318,6 +1576,48 @@ static int conv_tail(const void* x, const float* weight, const float* bias, cons
   return DINVK_POST_LAUNCH();
 }
 
+template <class F>
+static int conv_head3d(const float* x_ncdhw, const float* weight, const float* bias, void* out, int B, int C, int D, int H, int W, int Cout,
+                       float fill_scalar, const float* fill_batch, int has_fill, int act, int* flag, void* stream) {
+  const int CT = C + (has_fill ? 1 : 0);
+  DINVK_CHECK_ARG(Cout % F::CH == 0 && Cout >= F::CH && Cout <= 256, "conv3d_tc32_head: Cout=%d must be a multiple of %d (<= 256)", Cout, F::CH);
+  Head3Params P{};
+  static_cast<HeadParams&>(P) = HeadParams{x_ncdhw, weight, bias, out, B, C, H, W, Cout, fill_scalar, fill_batch, has_fill, act, flag};
+  P.D = D;
+  const long long npix = (long long)B * D * H * W;
+  DINVK_CHECK_ARG((npix + 255) / 256 < (1LL << 31), "conv3d_tc32_head: grid too large");
+  const unsigned grid = (unsigned)((npix + 255) / 256);
+  switch (CT) {
+    case 1: DINVK_LAUNCH((head3d_tc32_kernel<F, 1>), dim3(grid), dim3(256), 0, stream, P); break;
+    case 2: DINVK_LAUNCH((head3d_tc32_kernel<F, 2>), dim3(grid), dim3(256), 0, stream, P); break;
+    case 3: DINVK_LAUNCH((head3d_tc32_kernel<F, 3>), dim3(grid), dim3(256), 0, stream, P); break;
+    default: DINVK_LAUNCH((head3d_tc32_kernel<F, 4>), dim3(grid), dim3(256), 0, stream, P); break;
+  }
+  return DINVK_POST_LAUNCH();
+}
+
+template <class F>
+static int conv_tail3d(const void* x, const float* weight, const float* bias, const float* add_ncdhw, float* out_ncdhw, int B, int D, int H,
+                       int W, int Cin, int Cout, const int* flag, void* stream) {
+  DINVK_CHECK_ARG(Cin % F::CH == 0 && Cin >= F::CH && Cin <= 128, "conv3d_tc32_tail: Cin=%d must be a multiple of %d (<= 128)", Cin, F::CH);
+  Tail3Params P{};
+  static_cast<TailParams&>(P) = TailParams{x, weight, bias, add_ncdhw, out_ncdhw, B, H, W, Cin, Cout, flag};
+  P.D = D;
+  const long long tiles = (long long)B * D * ceil_div(H, TL_TY) * ceil_div(W, TL_TX);
+  DINVK_CHECK_ARG(tiles < (1LL << 31), "conv3d_tc32_tail: grid too large");
+  const int CO = Cout <= 2 ? 2 : 4;
+  const size_t smem = ((size_t)(TL_TY + 2) * (TL_TX + 2) * (TL3_CC + 4) + (size_t)CO * 27 * Cin) * 4;
+  int rc;
+  if (CO == 2) {
+    if ((rc = allow_smem(tail3d_tc32_kernel<F, 2>, smem))) return rc;
+    DINVK_LAUNCH((tail3d_tc32_kernel<F, 2>), dim3((unsigned)tiles), dim3(256), smem, stream, P);
+  } else {
+    if ((rc = allow_smem(tail3d_tc32_kernel<F, 4>, smem))) return rc;
+    DINVK_LAUNCH((tail3d_tc32_kernel<F, 4>), dim3((unsigned)tiles), dim3(256), smem, stream, P);
+  }
+  return DINVK_POST_LAUNCH();
+}
+
 }  // namespace t32
 }  // namespace dinvk
 
@@ -1346,7 +1646,39 @@ extern "C" int dinvk_conv_tc32_slab(const void* x, const void* weight, const flo
                      conv_slab<FmtF16>(x, weight, bias, res, res2, out, B, H, W, Cin, Cout, act, window, overflow_flag, stream));
 }
 
+extern "C" int dinvk_conv3d_tc32(const void* x, const void* weight, const float* bias, const void* res, const void* res2, void* out, int B,
+                                 int D, int H, int W, int Cin, int Cout, int kind, int act, int window, int fmt, int* overflow_flag,
+                                 void* stream) {
+  using namespace t32;
+  DINVK_FMT_DISPATCH(fmt, conv_generic3d<FmtTF32>(x, weight, bias, res, res2, out, B, D, H, W, Cin, Cout, kind, act, window, overflow_flag, stream),
+                     conv_generic3d<FmtF16>(x, weight, bias, res, res2, out, B, D, H, W, Cin, Cout, kind, act, window, overflow_flag, stream));
+}
+
 #endif  // !DINVK_EMUL
+extern "C" int dinvk_conv3d_tc32_head(const float* x_ncdhw, const float* weight, const float* bias, void* out, int B, int C, int D, int H,
+                                      int W, int Cout, float fill_scalar, const float* fill_batch, int has_fill, int act, int fmt,
+                                      int* overflow_flag, void* stream) {
+  using namespace t32;
+  DINVK_CHECK_ARG(x_ncdhw && weight && out && B >= 0 && C >= 1 && D >= 1 && H >= 1 && W >= 1, "conv3d_tc32_head: bad arguments");
+  const int CT = C + (has_fill ? 1 : 0);
+  DINVK_CHECK_ARG(CT >= 1 && CT <= 4, "conv3d_tc32_head: %d input channels (incl. noise map) not in 1..4", CT);
+  DINVK_CHECK_ARG(product_fits(B, D, H, W, 4, std::max(Cout, 4)), "conv3d_tc32_head: volume (%d, %d, %d, %d) too large", B, D, H, W);
+  if (B == 0) return DINVK_OK;
+  DINVK_FMT_DISPATCH(fmt, conv_head3d<FmtTF32>(x_ncdhw, weight, bias, out, B, C, D, H, W, Cout, fill_scalar, fill_batch, has_fill, act, overflow_flag, stream),
+                     conv_head3d<FmtF16>(x_ncdhw, weight, bias, out, B, C, D, H, W, Cout, fill_scalar, fill_batch, has_fill, act, overflow_flag, stream));
+}
+
+extern "C" int dinvk_conv3d_tc32_tail(const void* x, const float* weight, const float* bias, const float* add_ncdhw, float* out_ncdhw, int B,
+                                      int D, int H, int W, int Cin, int Cout, int fmt, const int* overflow_flag, void* stream) {
+  using namespace t32;
+  DINVK_CHECK_ARG(x && weight && out_ncdhw && B >= 0 && D >= 1 && H >= 1 && W >= 1, "conv3d_tc32_tail: bad arguments");
+  DINVK_CHECK_ARG(Cout >= 1 && Cout <= 4, "conv3d_tc32_tail: Cout=%d not in 1..4", Cout);
+  DINVK_CHECK_ARG(product_fits(B, D, H, W, 4, std::max(Cin, 4)), "conv3d_tc32_tail: volume (%d, %d, %d, %d) too large", B, D, H, W);
+  if (B == 0) return DINVK_OK;
+  DINVK_FMT_DISPATCH(fmt, conv_tail3d<FmtTF32>(x, weight, bias, add_ncdhw, out_ncdhw, B, D, H, W, Cin, Cout, overflow_flag, stream),
+                     conv_tail3d<FmtF16>(x, weight, bias, add_ncdhw, out_ncdhw, B, D, H, W, Cin, Cout, overflow_flag, stream));
+}
+
 extern "C" int dinvk_conv_tc32_head(const float* x_nchw, const float* weight, const float* bias, void* out, int B, int C, int H, int W,
                                     int Cout, float fill_scalar, const float* fill_batch, int has_fill, int act, int fmt,
                                     int* overflow_flag, void* stream) {

@@ -71,6 +71,13 @@ __device__ __forceinline__ void tma_load_4d(void* smem, const CUtensorMap* m, ui
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
+__device__ __forceinline__ void tma_load_5d(void* smem, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2, int c3, int c4) {
+  asm volatile(
+      "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];" ::"r"(
+          smem_u32(smem)),
+      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
+      : "memory");
+}
 
 // ---- wgmma (Hopper warpgroup MMA) -------------------------------------------------------------------
 // D[registers] (+)= A[smem] * B[smem], both operands K-major with the 128-byte swizzle TMA writes.  Issued by all 128

@@ -238,6 +238,71 @@ def drunet_forward_tc32(model, x0: torch.Tensor) -> torch.Tensor:
     return ops.conv_tc32_tail(t, pk.tail, flag=f)
 
 
+# ---- DRUNet(dim=3): the same dataflow on NDHWC split volumes, every layer on the per-tap kernel (csrc/conv_tc32.cu, D3) ----
+def _pack3x3x3_tc32(w, fmt: int = 0):   # (Cout, Cin, 3, 3, 3) -> k = ((kz*3+ky)*3+kx)*Cin + c
+    return _pack_tc32(w.detach().float().permute(0, 2, 3, 4, 1).reshape(w.shape[0], -1), fmt)
+
+
+def _pack_down3d_tc32(w, fmt: int = 0):  # (Cout, Cin, 2, 2, 2) -> k = (dz*4+dy*2+dx)*Cin + c
+    return _pack_tc32(w.detach().float().permute(0, 2, 3, 4, 1).reshape(w.shape[0], -1), fmt)
+
+
+def _pack_up3d_tc32(w, fmt: int = 0):    # (Cin, Cout, 2, 2, 2) -> row = (dz*4+dy*2+dx)*Cout + co
+    return _pack_tc32(w.detach().float().permute(2, 3, 4, 1, 0).reshape(-1, w.shape[0]), fmt)
+
+
+class _Drunet3dPack32(_DrunetPack32):
+    def __init__(self, m, fmt):
+        from .drunet import body_blocks
+
+        nb = m.nb
+        self.key = (_version_key(m), fmt)
+        self.fmt = fmt
+        self.nc = [m.m_head.weight.shape[0], m.m_down1[nb].weight.shape[0], m.m_down2[nb].weight.shape[0],
+                   m.m_down3[nb].weight.shape[0]]
+        if any(c % 64 for c in self.nc) or m.m_head.weight.shape[1] > 4 or m.m_tail.weight.shape[0] > 4 or self.nc[0] > 128:
+            raise NotImplementedError("precision='tc32' / 'tc32h' need channel counts that are multiples of 64 (tensor-core N/K tiles), "
+                                      f"at most 4 image channels and nc[0] <= 128; got nc={self.nc}; use precision='fp32'")
+        self.head = m.m_head.weight.detach().float().contiguous()
+        self.tail = m.m_tail.weight.detach().float().contiguous()
+        self.flag = torch.zeros(1, dtype=torch.int32, device=self.head.device)
+        rb = lambda blocks: [(_pack3x3x3_tc32(b.res[0].weight, fmt), _pack3x3x3_tc32(b.res[2].weight, fmt), b.res[0].weight.shape[0])
+                             for b in blocks]
+        self.down = [(rb(list(st)[:nb]), _pack_down3d_tc32(st[nb].weight, fmt), st[nb].weight.shape[0]) for st in (m.m_down1, m.m_down2, m.m_down3)]
+        self.body = rb(body_blocks(m))
+        self.up = [(_pack_up3d_tc32(st[0].weight, fmt), st[0].weight.shape[1], rb(list(st)[1:])) for st in (m.m_up3, m.m_up2, m.m_up1)]
+
+
+def _resblocks3d32(t, blocks, flag, skip=None):
+    for i, (w0, w1, c) in enumerate(blocks):
+        u = ops.conv3d_tc32(t, w0, c, relu=True, flag=flag)
+        t = ops.conv3d_tc32(u, w1, c, res=t, res2=skip if i == len(blocks) - 1 else None, flag=flag)
+    return t
+
+
+def drunet3d_forward_tc32(model, x0: torch.Tensor) -> torch.Tensor:
+    """x0: (B, C+1, D, H, W) fp32 (noise map already concatenated) -> (B, C_out, D, H, W) fp32; the dataflow of drunet_forward_tc32"""
+    fmt = _fmt(model.precision)
+    pk = model._tc32
+    if not isinstance(pk, _Drunet3dPack32) or pk.key != (_version_key(model), fmt):
+        pk = model._tc32 = _Drunet3dPack32(model, fmt)
+    f = pk.flag if fmt == 1 else None
+    if f is not None:
+        f.zero_()   # the flag is per call: an out-of-range input poisons its own output, not the model
+    x1 = ops.conv3d_tc32_head(x0, pk.head, fmt=fmt, flag=f)
+    skips = [x1]
+    t = x1
+    for blocks, wd, cd in pk.down:
+        t = _resblocks3d32(t, blocks, f)
+        t = ops.conv3d_tc32(t, wd, cd, kind=1, flag=f)
+        skips.append(t)
+    t = _resblocks3d32(t, pk.body, f, skip=skips[3])
+    for i, (wu, cu, blocks) in enumerate(pk.up):
+        t = ops.conv3d_tc32(t, wu, cu, kind=2, flag=f)
+        t = _resblocks3d32(t, blocks, f, skip=skips[2 - i])
+    return ops.conv3d_tc32_tail(t, pk.tail, flag=f)
+
+
 class _DncnnPack32:
     def __init__(self, m, fmt):
         self.key = (_version_key(m), fmt)

@@ -749,6 +749,75 @@ def conv_tc32_tail(x, weight, *, bias=None, add=None, flag=None) -> torch.Tensor
     return out
 
 
+def conv3d_f32(x, weight, *, kind: int = 0, bias=None, xadd=None, res=None, relu: bool = False) -> torch.Tensor:
+    """3-D `conv_f32` on (B, C, D, H, W): kind 0: 3x3x3 pad 1, 1: 2x2x2 stride 2, 2: transposed 2x2x2 stride 2 (forward only)"""
+    dev = _require_cuda(x, weight, bias, xadd, res)
+    x, weight, bias, xadd, res = _f32c(x), _f32c(weight), _f32c(bias), _f32c(xadd), _f32c(res)
+    B, Cin, D, H, W = x.shape
+    Cout = weight.shape[1] if kind == 2 else weight.shape[0]
+    scale = {0: (1, 1), 1: (1, 2), 2: (2, 1)}.get(kind, (1, 1))
+    out = torch.empty(B, Cout, *(s * scale[0] // scale[1] for s in (D, H, W)), dtype=torch.float32, device=dev)
+    if out.numel() == 0:
+        return out
+    check(get_lib().dinvk_conv3d_f32(_p(x), _p(xadd), _p(weight), _p(bias), _p(res), _p(out), B, Cin, Cout, D, H, W, kind,
+                                     int(relu), _stream(dev)))
+    return out
+
+
+def _split3d_empty(B, D, H, W, C, fmt, dev):
+    ch, dt = (32, torch.float16) if fmt == 1 else (16, torch.float32)
+    return torch.empty(B, D, H, W, C // ch, 2, ch, dtype=dt, device=dev)
+
+
+def conv3d_tc32(x, w, cout: int, *, kind: int = 0, bias=None, res=None, res2=None, relu: bool = False, window: int = 0,
+                flag=None) -> torch.Tensor:
+    """x split volume (B, D, H, W, C/CH, 2, CH), w packed by models.tc_engine (27-tap, 2x2x2 down or up order) -> split output
+    kind 0: 3x3x3 (same grid), 1: 2x2x2 stride 2, 2: transposed 2x2x2 stride 2;  out = act(conv + bias) + res + res2"""
+    dev = _require_cuda(x, w)
+    fmt = _fmt_of(x)
+    B, D, H, W, nblk = x.shape[:5]
+    Cin = nblk * x.shape[-1]
+    f = {0: lambda s: s, 1: lambda s: s // 2, 2: lambda s: 2 * s}.get(kind, lambda s: s)
+    out = _split3d_empty(B, f(D), f(H), f(W), cout, fmt, dev)
+    if out.numel() == 0:
+        return out
+    check(get_lib().dinvk_conv3d_tc32(_p(x), _p(w), _p(bias), _p(res), _p(res2), _p(out), B, D, H, W, Cin, cout, kind, int(relu),
+                                      int(window), fmt, _p(flag), _stream(dev)))
+    return out
+
+
+def conv3d_tc32_head(x, weight, *, bias=None, fill=None, relu: bool = False, fmt: int = 0, flag=None) -> torch.Tensor:
+    """3-D network head: (B,C,D,H,W) fp32 (+ constant channel `fill`) -> split volume; weight (Cout,C[+1],3,3,3) fp32"""
+    dev = _require_cuda(x, weight)
+    x = _f32c(x)
+    B, C, D, H, W = x.shape
+    cout = weight.shape[0]
+    out = _split3d_empty(B, D, H, W, cout, fmt, dev)
+    fill_t = _f32c(fill.reshape(-1)) if torch.is_tensor(fill) else None
+    if fill_t is not None and fill_t.numel() == 1:
+        fill_t = fill_t.expand(B).contiguous()
+    if out.numel() == 0:
+        return out
+    check(get_lib().dinvk_conv3d_tc32_head(_p(x), _p(_f32c(weight)), _p(bias), _p(out), B, C, D, H, W, cout,
+                                           float(fill) if (fill is not None and fill_t is None) else 0.0,
+                                           _p(fill_t), int(fill is not None), int(relu), fmt, _p(flag), _stream(dev)))
+    return out
+
+
+def conv3d_tc32_tail(x, weight, *, bias=None, add=None, flag=None) -> torch.Tensor:
+    """3-D network tail: split volume -> (B,Cout,D,H,W) fp32 (+ bias + add); weight (Cout,Cin,3,3,3) fp32, Cout <= 4;
+    NaN if the network's overflow flag is set"""
+    dev = _require_cuda(x, weight)
+    B, D, H, W, nblk = x.shape[:5]
+    cout = weight.shape[0]
+    out = torch.empty(B, cout, D, H, W, dtype=torch.float32, device=dev)
+    if out.numel() == 0:
+        return out
+    check(get_lib().dinvk_conv3d_tc32_tail(_p(x), _p(_f32c(weight)), _p(bias), _p(_f32c(add)), _p(out), B, D, H, W, nblk * x.shape[-1],
+                                           cout, _fmt_of(x), _p(flag), _stream(dev)))
+    return out
+
+
 def split16_to_nchw(x) -> torch.Tensor:
     dev = _require_cuda(x)
     B, H, W, nblk = x.shape[:4]

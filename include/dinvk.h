@@ -363,9 +363,32 @@ int dinvk_conv_tc32_head(const float* x_nchw, const float* weight, const float* 
 int dinvk_conv_tc32_tail(const void* x, const float* weight, const float* bias, const float* add_nchw,
                          float* out_nchw, int B, int H, int W, int Cin, int Cout, int fmt, const int* overflow_flag,
                          void* stream);
-/* layout converters split <-> NCHW fp32 (C % CH == 0) */
+/* layout converters split <-> NCHW fp32 (C % CH == 0); called with H' = D*H they convert NDHWC split volumes <-> NCDHW */
 int dinvk_split16_to_nchw(const void* in, float* out, int B, int C, int H, int W, int fmt, void* stream);
 int dinvk_nchw_to_split16(const float* in, void* out, int B, int C, int H, int W, int fmt, void* stream);
+
+/* 3-D denoiser convolutions (DRUNet(dim=3): deepinv/models/drunet.py with Conv3d / ConvTranspose3d), forward only.
+ * fp32 CUDA-core path, NCDHW:  kind 0: 3x3x3 stride 1 zero-pad 1, weight (Cout,Cin,3,3,3);  kind 1: 2x2x2 stride 2 (D, H, W
+ *   even), weight (Cout,Cin,2,2,2);  kind 2: transposed 2x2x2 stride 2, weight (Cin,Cout,2,2,2);
+ *   out = act(conv(x [+ xadd]) + bias) + res, as dinvk_conv_f32. */
+int dinvk_conv3d_f32(const float* x, const float* xadd, const float* weight, const float* bias, const float* res,
+                     float* out, int B, int Cin, int Cout, int D, int H, int W, int kind, int act, void* stream);
+/* split-operand wgmma path on NDHWC split volumes (B,D,H,W,C/CH,2,CH), formats and weight rows as dinvk_conv_tc32:
+ *   kind 0 (3x3x3, pad 1): (2*Cout, 27*Cin), k = ((kz*3+ky)*3+kx)*Cin + c
+ *   kind 1 (2x2x2 stride 2): (2*Cout, 8*Cin), k = (dz*4+dy*2+dx)*Cin + c;  out (B,D/2,H/2,W/2,Cout)
+ *   kind 2 (transposed 2x2x2 stride 2): (16*Cout, Cin), GEMM column = (dz*4+dy*2+dx)*Cout + co;  out (B,2D,2H,2W,Cout)
+ *   out = act(conv(x) + bias) + res + res2 (kind 0 only).  Cin % (2 CH) == 0, Cout % 64 == 0. */
+int dinvk_conv3d_tc32(const void* x, const void* weight, const float* bias, const void* res, const void* res2, void* out,
+                      int B, int D, int H, int W, int Cin, int Cout, int kind, int act, int window, int fmt,
+                      int* overflow_flag, void* stream);
+/* 3-D head: NCDHW fp32 volume (+ optional constant noise-level channel) -> split NDHWC; weight (Cout, C + has_fill, 3,3,3) */
+int dinvk_conv3d_tc32_head(const float* x_ncdhw, const float* weight, const float* bias, void* out, int B, int C, int D,
+                           int H, int W, int Cout, float fill_scalar, const float* fill_batch, int has_fill, int act,
+                           int fmt, int* overflow_flag, void* stream);
+/* 3-D tail: split NDHWC -> NCDHW fp32, Cout <= 4;  out = conv3x3x3(x) + bias + add_ncdhw;  NaN if *overflow_flag is set */
+int dinvk_conv3d_tc32_tail(const void* x, const float* weight, const float* bias, const float* add_ncdhw,
+                           float* out_ncdhw, int B, int D, int H, int W, int Cin, int Cout, int fmt,
+                           const int* overflow_flag, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Total variation (2-D, images (B,C,H,W) fp32; gradient fields (B,C,H,W,2), component 0 vertical)
