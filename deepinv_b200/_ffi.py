@@ -64,6 +64,9 @@ _SIGNATURES = {
     "dinvk_svblur_adj": (c_int, [c_void_p] * 4 + [c_int] * 12 + [c_void_p, c_size_t, c_void_p]),
     "dinvk_tiled_svblur_fwd": (c_int, [c_void_p] * 4 + [c_int] * 13 + [c_void_p]),
     "dinvk_tiled_svblur_adj": (c_int, [c_void_p] * 4 + [c_int] * 13 + [c_void_p]),
+    "dinvk_resize_fwd": (c_int, [c_void_p] * 2 + [c_int] * 5 + [c_void_p] * 2 + [c_int] + [c_void_p] * 2 + [c_int, C.c_double,
+                                                                                                      c_void_p]),
+    "dinvk_resize_adj": (c_int, [c_void_p] * 2 + [c_int] * 5 + [c_void_p] * 6 + [c_int, C.c_double, c_void_p]),
     "dinvk_conv_f32": (c_int, [c_void_p] * 6 + [c_int] * 7 + [c_void_p]),
     "dinvk_conv_f32_wgrad": (c_int, [c_void_p] * 5 + [c_int] * 6 + [c_void_p]),
     "dinvk_relu_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),

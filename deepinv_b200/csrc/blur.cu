@@ -1176,3 +1176,212 @@ extern "C" int dinvk_blur3d_adj(const float* y, const float* filt, float* x, int
                padding == DINVK_PAD_REPLICATE ? 2 : 3);
   return DINVK_POST_LAUNCH();
 }
+
+// ---- MATLAB-bicubic resize: deepinv/physics/functional/imresize.py:222-296 (resize_1d) applied to H then W, the body of
+// imresize_matlab (:299-372) and of DownsamplingMatlab.A (deepinv/physics/blur.py:1195-1261), and its exact transpose
+// (DownsamplingMatlab.A_adjoint, which the reference computes by autograd) ----------------------------------------------
+// Per plane y = M_H x M_W^T, with M (n_out x n_in) banded: output o reads the k taps base[o] + t (t < k) of the input axis,
+// reflected MATLAB-style (j < 0 -> -1 - j, j >= n -> 2n - 1 - j: the edge sample repeated), weighted by w[o*k + t].  The
+// tables (unreflected base, fp32 weights; the transpose's CSR by input index) are built by the caller with the reference's
+// own arithmetic.
+//   forward   : a CTA owns RS_TH output rows x TW output columns of one plane.  The H pass gathers, for each of its rows and
+//               each input column the W band of the tile reaches, the k_h taps of x (through L1) into shared memory; the W
+//               pass then sums k_w taps of that intermediate per output.  Nothing goes to HBM between the passes.
+//   transpose : gather form.  A CTA owns RS_TH input rows x TW input columns.  The H^T pass sums, per row, the CSR entries of
+//               M_H^T over the y rows (read through L1) for each y column the tile's W^T band reaches; the W^T pass sums the
+//               CSR entries of M_W^T over that intermediate.  Reflection folds stay separate entries.
+// Every sum runs in table order with each product and sum rounded separately: no atomics, bitwise reproducible.
+namespace dinvk {
+
+constexpr int RS_TH = 16;
+constexpr size_t RS_SMEM_BUDGET = 96 * 1024;
+
+struct ResizeParams {
+  int H, W, Ho, Wo;   // input (H, W), output (Ho, Wo) of the forward
+  int kh, kw;         // taps per output (forward only)
+  int TW, cap;        // tile columns; row pitch of the intermediate (columns it can hold)
+  int tiles_x, BC;
+};
+
+__device__ __forceinline__ int rs_reflect(int j, int n) {
+  j = j < 0 ? -1 - j : (j >= n ? 2 * n - 1 - j : j);
+  return min(max(j, 0), n - 1);  // a table the builder would have refused (pad > n) stays in bounds
+}
+
+__global__ void __launch_bounds__(256) resize_fwd_kernel(const float* __restrict__ x, float* __restrict__ y,
+                                                         const int* __restrict__ base_h, const float* __restrict__ wt_h,
+                                                         const int* __restrict__ base_w, const float* __restrict__ wt_w,
+                                                         ResizeParams P) {
+  DINVK_DYN_SMEM(float, sm);
+  const int TW = P.TW, kh = P.kh, kw = P.kw;
+  float* tmp = sm;                                              // [RS_TH][cap]  the H pass
+  float* whs = tmp + RS_TH * P.cap;                             // [RS_TH][kh]   H weights of the tile's rows
+  int* rows = reinterpret_cast<int*>(whs + RS_TH * kh);         // [RS_TH][kh]   their reflected input rows
+  float* wws = reinterpret_cast<float*>(rows + RS_TH * kh);     // [kw][TW]      W weights, tap-major
+  int* offs = reinterpret_cast<int*>(wws + kw * TW);            // [TW]          first tap of each column in tmp
+  const int ty = blockIdx.x / P.tiles_x, tx = blockIdx.x - ty * P.tiles_x;
+  const int oh0 = ty * RS_TH, ow0 = tx * TW;
+  const int nr = min(RS_TH, P.Ho - oh0), nq = min(TW, P.Wo - ow0);
+  const int c0 = __ldg(base_w + ow0);
+  const int span = max(1, min(__ldg(base_w + ow0 + nq - 1) + kw - c0, P.cap));
+  for (int i = threadIdx.x; i < nr * kh; i += 256) {
+    const int r = i / kh, t = i - r * kh;
+    whs[i] = __ldg(wt_h + (long long)(oh0 + r) * kh + t);
+    rows[i] = rs_reflect(__ldg(base_h + oh0 + r) + t, P.H);
+  }
+  for (int i = threadIdx.x; i < nq * kw; i += 256) {
+    const int q = i / kw, t = i - q * kw;
+    wws[t * TW + q] = __ldg(wt_w + (long long)(ow0 + q) * kw + t);
+  }
+  for (int q = threadIdx.x; q < nq; q += 256) offs[q] = __ldg(base_w + ow0 + q) - c0;
+  __syncthreads();
+  for (int bc = blockIdx.y; bc < P.BC; bc += gridDim.y) {
+    const float* xp = x + (long long)bc * P.H * P.W;
+    for (int i = threadIdx.x; i < nr * span; i += 256) {
+      const int r = i / span, c = i - r * span;
+      const float* xc = xp + rs_reflect(c0 + c, P.W);
+      const float* wr = whs + r * kh;
+      const int* rr = rows + r * kh;
+      float acc = 0.f;
+      for (int t = 0; t < kh; ++t) acc = __fadd_rn(acc, __fmul_rn(__ldg(xc + (long long)rr[t] * P.W), wr[t]));
+      tmp[r * P.cap + c] = acc;
+    }
+    __syncthreads();
+    float* yp = y + (long long)bc * P.Ho * P.Wo;
+    for (int i = threadIdx.x; i < nr * nq; i += 256) {
+      const int r = i / nq, q = i - r * nq;
+      const float* tr = tmp + r * P.cap;
+      const int o = offs[q];
+      float acc = 0.f;
+      for (int t = 0; t < kw; ++t) acc = __fadd_rn(acc, __fmul_rn(tr[min(max(o + t, 0), span - 1)], wws[t * TW + q]));
+      yp[(long long)(oh0 + r) * P.Wo + ow0 + q] = acc;
+    }
+    __syncthreads();
+  }
+}
+
+__global__ void __launch_bounds__(256) resize_adj_kernel(const float* __restrict__ y, float* __restrict__ x,
+                                                         const int* __restrict__ ptr_h, const int* __restrict__ out_h,
+                                                         const float* __restrict__ wt_h, const int* __restrict__ ptr_w,
+                                                         const int* __restrict__ out_w, const float* __restrict__ wt_w,
+                                                         ResizeParams P) {
+  DINVK_DYN_SMEM(float, tmp);  // [RS_TH][cap]: the H^T pass over the y columns the tile's W^T band reaches
+  __shared__ int range[2];
+  const int TW = P.TW;
+  const int ty = blockIdx.x / P.tiles_x, tx = blockIdx.x - ty * P.tiles_x;
+  const int ih0 = ty * RS_TH, iw0 = tx * TW;
+  const int nr = min(RS_TH, P.H - ih0), nq = min(TW, P.W - iw0);
+  if (threadIdx.x < 32) {  // y columns [lo, hi] the tile's columns gather from (CSR rows are sorted by output index)
+    int lo = 2147483647, hi = -1;
+    for (int q = threadIdx.x; q < nq; q += 32) {
+      const int a = __ldg(ptr_w + iw0 + q), b = __ldg(ptr_w + iw0 + q + 1);
+      if (b > a) { lo = min(lo, __ldg(out_w + a)); hi = max(hi, __ldg(out_w + b - 1)); }
+    }
+    for (int m = 16; m; m >>= 1) {
+      lo = min(lo, __shfl_xor_sync(0xffffffffu, lo, m));
+      hi = max(hi, __shfl_xor_sync(0xffffffffu, hi, m));
+    }
+    if (threadIdx.x == 0) { range[0] = lo; range[1] = hi; }
+  }
+  __syncthreads();
+  const int olo = range[0], span = range[1] >= olo ? min(range[1] - olo + 1, P.cap) : 0;
+  for (int bc = blockIdx.y; bc < P.BC; bc += gridDim.y) {
+    const float* yp = y + (long long)bc * P.Ho * P.Wo;
+    for (int i = threadIdx.x; i < nr * span; i += 256) {
+      const int r = i / span, c = i - r * span;
+      const int a = __ldg(ptr_h + ih0 + r), b = __ldg(ptr_h + ih0 + r + 1);
+      const float* yc = yp + min(olo + c, P.Wo - 1);
+      float acc = 0.f;
+      for (int e = a; e < b; ++e)
+        acc = __fadd_rn(acc, __fmul_rn(__ldg(yc + (long long)min(max(__ldg(out_h + e), 0), P.Ho - 1) * P.Wo), __ldg(wt_h + e)));
+      tmp[r * P.cap + c] = acc;
+    }
+    __syncthreads();
+    float* xp = x + (long long)bc * P.H * P.W;
+    for (int i = threadIdx.x; i < nr * nq; i += 256) {
+      const int r = i / nq, q = i - r * nq;
+      const int a = __ldg(ptr_w + iw0 + q), b = __ldg(ptr_w + iw0 + q + 1);
+      const float* tr = tmp + r * P.cap;
+      float acc = 0.f;
+      for (int e = a; e < b; ++e) acc = __fadd_rn(acc, __fmul_rn(tr[min(max(__ldg(out_w + e) - olo, 0), span - 1)], __ldg(wt_w + e)));
+      xp[(long long)(ih0 + r) * P.W + iw0 + q] = acc;
+    }
+    __syncthreads();
+  }
+}
+
+// Columns of the intermediate a tile can need, from the resize scale s (output / input length) of the W axis:
+//   forward   : TW consecutive outputs start (TW - 1) / s input samples apart, plus k taps (+2 for the fp32 rounding of pos);
+//   transpose : the outputs whose band reaches TW consecutive inputs or their reflections, at most (TW + 3k + 2) s + 4 of them.
+static int resize_cap(bool fwd, int TW, double s, int k, int n_out) {
+  if (fwd) return (int)std::min(1e9, std::floor((TW - 1) / s)) + k + 2;
+  return (int)std::min<double>(n_out, std::floor((TW + 3.0 * k + 2) * s) + 4);
+}
+
+static size_t resize_smem(bool fwd, const ResizeParams& P) {
+  return fwd ? sizeof(float) * ((size_t)RS_TH * P.cap + 2 * (size_t)RS_TH * P.kh + (size_t)P.kw * P.TW + P.TW)
+             : sizeof(float) * (size_t)RS_TH * P.cap;
+}
+
+// tile width: 64 columns, halved until the intermediate and the tables fit the shared-memory budget
+static int resize_plan(bool fwd, int BC, int H, int W, int Ho, int Wo, int kh, int kw, double sw, ResizeParams* P, size_t* smem,
+                       dim3* grid) {
+  P->H = H; P->W = W; P->Ho = Ho; P->Wo = Wo; P->kh = kh; P->kw = kw; P->BC = BC;
+  const int ncol = fwd ? Wo : W, nrow = fwd ? Ho : H;
+  for (int TW = 64;; TW >>= 1) {
+    P->TW = TW;
+    P->cap = resize_cap(fwd, std::min(TW, ncol), sw, kw, Wo);
+    *smem = resize_smem(fwd, *P);
+    if (*smem <= RS_SMEM_BUDGET) break;
+    if (TW == 1) return set_error(DINVK_EUNSUPPORTED, "resize: a %d-tap band at scale %g does not fit the tiled kernel", kw, sw);
+  }
+  P->tiles_x = ceil_div(ncol, P->TW);
+  const long long tiles = (long long)P->tiles_x * ceil_div(nrow, RS_TH);
+  if (tiles > 2147483647LL) return set_error(DINVK_EINVAL, "resize: grid too large");
+  *grid = dim3((unsigned)tiles, (unsigned)std::min(BC, 65535));
+  return DINVK_OK;
+}
+
+static int check_resize_args(const void* in, const void* out, const void* t0, const void* t1, const void* t2, const void* t3,
+                             int BC, int H, int W, int Ho, int Wo, double sw) {
+  DINVK_CHECK_ARG(in && out, "resize: null pointer");
+  DINVK_CHECK_ARG(t0 && t1 && t2 && t3, "resize: null table");
+  DINVK_CHECK_ARG(BC >= 0 && H >= 1 && W >= 1 && Ho >= 1 && Wo >= 1, "resize: bad shape (%d, %d, %d) -> (%d, %d)", BC, H, W, Ho, Wo);
+  DINVK_CHECK_ARG(std::isfinite(sw) && sw > 0, "resize: bad scale %g", sw);
+  DINVK_CHECK_ARG(product_fits(BC, H, W) && product_fits(BC, Ho, Wo), "resize: tensor too large");
+  return DINVK_OK;
+}
+
+}  // namespace dinvk
+
+extern "C" int dinvk_resize_fwd(const float* x, float* y, int BC, int H, int W, int Ho, int Wo, const int* base_h, const float* wt_h,
+                                int kh, const int* base_w, const float* wt_w, int kw, double scale_w, void* stream) {
+  int rc = check_resize_args(x, y, base_h, wt_h, base_w, wt_w, BC, H, W, Ho, Wo, scale_w);
+  if (rc) return rc;
+  DINVK_CHECK_ARG(kh >= 1 && kw >= 1, "resize: bad tap counts (%d, %d)", kh, kw);
+  if (BC == 0) return DINVK_OK;
+  ResizeParams P;
+  size_t smem;
+  dim3 grid;
+  if ((rc = resize_plan(true, BC, H, W, Ho, Wo, kh, kw, scale_w, &P, &smem, &grid))) return rc;
+  if ((rc = allow_smem(resize_fwd_kernel, smem))) return rc;
+  DINVK_LAUNCH(resize_fwd_kernel, grid, dim3(256), smem, stream, x, y, base_h, wt_h, base_w, wt_w, P);
+  return DINVK_POST_LAUNCH();
+}
+
+extern "C" int dinvk_resize_adj(const float* y, float* x, int BC, int H, int W, int Ho, int Wo, const int* ptr_h, const int* out_h,
+                                const float* wt_h, const int* ptr_w, const int* out_w, const float* wt_w, int kw, double scale_w,
+                                void* stream) {
+  int rc = check_resize_args(y, x, ptr_h, out_h, ptr_w, out_w, BC, H, W, Ho, Wo, scale_w);
+  if (rc) return rc;
+  DINVK_CHECK_ARG(wt_h && wt_w, "resize: null table");
+  DINVK_CHECK_ARG(kw >= 1, "resize: bad tap count %d", kw);
+  if (BC == 0) return DINVK_OK;
+  ResizeParams P;
+  size_t smem;
+  dim3 grid;
+  if ((rc = resize_plan(false, BC, H, W, Ho, Wo, 1, kw, scale_w, &P, &smem, &grid))) return rc;
+  if ((rc = allow_smem(resize_adj_kernel, smem))) return rc;
+  DINVK_LAUNCH(resize_adj_kernel, grid, dim3(256), smem, stream, y, x, ptr_h, out_h, wt_h, ptr_w, out_w, wt_w, P);
+  return DINVK_POST_LAUNCH();
+}

@@ -474,6 +474,43 @@ def ramp_filter(sino_am) -> torch.Tensor:
 
 
 # --------------------------------------------------------------------------------------------
+# MATLAB-bicubic resize (csrc/blur.cu: resize_fwd_kernel / resize_adj_kernel); tables from physics/imresize.py
+# --------------------------------------------------------------------------------------------
+def resize_fwd(x, th, tw) -> torch.Tensor:
+    """(B,C,H,W) -> (B,C,th.n_out,tw.n_out): both 1-D passes of the banded resize in one launch"""
+    dev = _require_cuda(x)
+    x = _f32c(x)
+    B, C, H, W = x.shape
+    if (H, W) != (th.n_in, tw.n_in):
+        raise ValueError(f"resize: tables for a {th.n_in}x{tw.n_in} image, got {H}x{W}")
+    y = torch.empty(B, C, th.n_out, tw.n_out, dtype=torch.float32, device=dev)
+    if y.numel() == 0:
+        return y
+    bh, wh = th.on(dev)[:2]
+    bw, ww = tw.on(dev)[:2]
+    check(get_lib().dinvk_resize_fwd(_p(x), _p(y), B * C, H, W, th.n_out, tw.n_out, _p(bh), _p(wh), th.k, _p(bw), _p(ww), tw.k,
+                                     tw.scale, _stream(dev)))
+    return y
+
+
+def resize_adj(y, th, tw) -> torch.Tensor:
+    """the transpose of resize_fwd: (B,C,th.n_out,tw.n_out) -> (B,C,th.n_in,tw.n_in)"""
+    dev = _require_cuda(y)
+    y = _f32c(y)
+    B, C, Ho, Wo = y.shape
+    if (Ho, Wo) != (th.n_out, tw.n_out):
+        raise ValueError(f"resize: tables for a {th.n_out}x{tw.n_out} measurement, got {Ho}x{Wo}")
+    x = torch.empty(B, C, th.n_in, tw.n_in, dtype=torch.float32, device=dev)
+    if x.numel() == 0:
+        return x
+    ph, oh, wh = th.on(dev)[2:]
+    pw, ow, ww = tw.on(dev)[2:]
+    check(get_lib().dinvk_resize_adj(_p(y), _p(x), B * C, th.n_in, tw.n_in, Ho, Wo, _p(ph), _p(oh), _p(wh), _p(pw), _p(ow), _p(ww),
+                                     tw.k, tw.scale, _stream(dev)))
+    return x
+
+
+# --------------------------------------------------------------------------------------------
 # Blur (direct convolution)
 # --------------------------------------------------------------------------------------------
 def blur_fwd(x, filt, padding: int) -> torch.Tensor:

@@ -1,5 +1,6 @@
 from . import functional, generator  # noqa: F401
-from .blur import Blur, BlurFFT, Downsampling, SpaceVaryingBlur, TiledSpaceVaryingBlur  # noqa: F401
+from .blur import (Blur, BlurFFT, Downsampling, DownsamplingMatlab, SpaceVaryingBlur, TiledSpaceVaryingBlur,  # noqa: F401
+                   Upsampling)
 from .forward import DecomposablePhysics, LinearPhysics, Physics  # noqa: F401
 from .mri import MRI, DynamicMRI, MRIMixin, MultiCoilMRI, SequentialMRI, TimeMixin  # noqa: F401
 from .noise import GaussianNoise, NoiseModel, ZeroNoise  # noqa: F401

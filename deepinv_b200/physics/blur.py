@@ -597,3 +597,82 @@ class Downsampling(LinearPhysics):
         rp = torch.stack([rc.real, rc.imag], 2).reshape(B * C, 2, H, W).contiguous()
         r = ops.spectral(rp, H, W, fwd=False, inv=True, centered=False)[:, 0].reshape(B, C, H, W)
         return ops.axpbypcz(z_hat, g, r, -g)
+
+
+class Upsampling(Downsampling):
+    r"""x = h^T * S^T (y): the transpose of `Downsampling` used as the forward operator (blur.py:392-440).  `A` is
+    Downsampling.A_adjoint and `A_adjoint` is Downsampling.A, on the same kernels; ``img_size`` is the (C, H, W) of the
+    upsampled image."""
+
+    def __init__(self, img_size, filter=None, factor: int = 2, padding: str = "circular", device="cpu", **kwargs):
+        assert padding != "valid", "Padding 'valid' is not supported for Upsampling operator."
+        super().__init__(img_size=img_size, filter=filter, factor=factor, padding=padding, device=device, **kwargs)
+
+    def A(self, x: Tensor, **kwargs) -> Tensor:
+        return super().A_adjoint(x, **kwargs)
+
+    def A_adjoint(self, y: Tensor, **kwargs) -> Tensor:
+        return super().A(y, **kwargs)
+
+    def prox_l2(self, z: Tensor, y: Tensor, gamma, use_fft: bool = True, **kwargs) -> Tensor:
+        # Downsampling's closed form with the roles swapped: the reference multiplies the spectrum of the (C, H, W) image size
+        # by that of z, which lives on the small grid, and fails on the size mismatch
+        if use_fft and self.padding == "circular" and self.filter is not None:
+            H, W = self.imsize[-2:]
+            if tuple(z.shape[-2:]) != (H, W):
+                dim = 3 if z.shape[-1] != W else 2
+                raise RuntimeError(f"The size of tensor a ({(H, W)[dim - 2]}) must match the size of tensor b "
+                                   f"({z.shape[dim]}) at non-singleton dimension {dim}")
+        return super().prox_l2(z, y, gamma, use_fft=use_fft, **kwargs)
+
+
+class DownsamplingMatlab(Downsampling):
+    r"""MATLAB ``imresize(x, 1 / factor, 'bicubic')``: the antialiased cubic kernel with reflect padding (blur.py:1195-1261).
+
+    `A` is one launch of the fused separable resize (`dinvk_resize_fwd`, csrc/blur.cu) and `A_adjoint` one launch of its exact
+    transpose (`dinvk_resize_adj`) on the (H_out f, W_out f) image, the domain on which the reference's autograd adjoint
+    lives.  The factor is truncated to an int as `Downsampling.check_factor` does, so a factor below 2 is the identity.
+    `A` is differentiable in x through the transpose kernel and `A_adjoint` in y through the forward kernel.  `prox_l2`,
+    `A_dagger` and the norm estimate are the inherited CG / power-method versions (reflect padding)."""
+
+    def __init__(self, factor=2, kernel: str = "cubic", padding: str = "reflect", antialiasing: bool = True, device="cpu",
+                 **kwargs):
+        super().__init__(filter=None, factor=factor, device=device, **kwargs)
+        self.kernel = kernel
+        self.padding = padding
+        self.antialiasing = antialiasing
+
+    def _plan(self, H: int, W: int):
+        from .imresize import resize_plan
+
+        return resize_plan(H, W, scale=1 / self.factor, antialiasing=self.antialiasing, kernel=self.kernel,
+                           padding_type=self.padding)
+
+    def A(self, x: Tensor, factor=None, **kwargs) -> Tensor:
+        from .imresize import resize
+
+        self.update_parameters(factor=factor, device=x.device, **kwargs)
+        if x.dim() not in (2, 3, 4):
+            raise ValueError("{}-dim Tensor is not supported!".format(x.dim()))
+        h, w = x.shape[-2:]
+        out, th, tw = self._plan(h, w)
+        if th is None and tw is None:
+            return x.clone()
+        return resize(x.reshape(-1, 1, h, w), th, tw).reshape(*x.shape[:-2], *out)
+
+    def A_adjoint(self, y: Tensor, factor=None, **kwargs) -> Tensor:
+        from .imresize import resize_adjoint
+
+        self.update_parameters(factor=factor, device=y.device, **kwargs)
+        if y.dim() != 4:
+            raise ValueError(f"Expected Tensor dimension to be 4, is {y.dim()}")
+        H, W = y.shape[-2] * self.factor, y.shape[-1] * self.factor
+        _, th, tw = self._plan(H, W)
+        return y.clone() if th is None and tw is None else resize_adjoint(y, th, tw, H, W)
+
+    def prox_l2(self, z: Tensor, y: Tensor, gamma, use_fft: bool = True, **kwargs) -> Tensor:
+        # reflect padding: the inherited CG route, which starts from A^T y + z / gamma.  A^T y lives on the (H_out f, W_out f)
+        # grid, so, as in the reference, an image whose sides are not multiples of the factor does not broadcast against it
+        if isinstance(z, Tensor):
+            torch.broadcast_shapes(tuple(z.shape), (*y.shape[:-2], y.shape[-2] * self.factor, y.shape[-1] * self.factor))
+        return super().prox_l2(z, y, gamma, use_fft=use_fft, **kwargs)

@@ -10,6 +10,8 @@ from math import exp, pi, sqrt
 
 import torch
 
+from .imresize import imresize_matlab  # noqa: F401
+
 
 def gaussian_blur(psf_size=None, sigma=(1.0, 1.0), angle=0.0, device="cpu", dtype=torch.float32) -> torch.Tensor:
     """2-D anisotropic, rotated Gaussian kernels (B,1,h,w), each normalised to sum 1 (functional/blur.py:137-264).

@@ -273,6 +273,23 @@ int dinvk_tiled_svblur_fwd(const float* x, const float* mult, const float* filt,
 int dinvk_tiled_svblur_adj(const float* y, const float* mult, const float* filt, float* x, int B, int C, int H, int W,
                            int FB, int FC, int K, int h, int w, int P1, int P2, int s1, int s2, void* stream);
 
+/* MATLAB-bicubic resize (deepinv/physics/functional/imresize.py:222-372, imresize_matlab with kernel 'cubic' and reflect
+ * padding; DownsamplingMatlab.A, deepinv/physics/blur.py:1195-1261) and its exact transpose (DownsamplingMatlab.A_adjoint).
+ * Per plane y = M_H x M_W^T: x (BC,H,W) -> y (BC,Ho,Wo).  Each axis is a banded matrix given by tables the caller builds:
+ *   forward  : base (n_out) int32, the first (unreflected) tap of each output, and weights (n_out, k) fp32; output o reads
+ *              input base[o] + t for t < k, reflected as j < 0 -> -1 - j, j >= n -> 2n - 1 - j (the caller guarantees that
+ *              the band reaches at most n samples past either edge);
+ *   transpose: the same matrix transposed, CSR by input index: ptr (n_in + 1), and per entry the output index (int32, sorted
+ *              ascending within a row) and weight (fp32).  Taps that reflection folds onto one input stay separate entries.
+ * kw and scale_w (Wo / W as the resize defines it, > 0) size the shared-memory band of a tile.  Each output sums its taps in
+ * table order with every product and sum rounded separately: one launch, no workspace, no atomics, bitwise reproducible.
+ * BC == 0 launches nothing. */
+int dinvk_resize_fwd(const float* x, float* y, int BC, int H, int W, int Ho, int Wo, const int* base_h, const float* wt_h,
+                     int kh, const int* base_w, const float* wt_w, int kw, double scale_w, void* stream);
+int dinvk_resize_adj(const float* y, float* x, int BC, int H, int W, int Ho, int Wo, const int* ptr_h, const int* out_h,
+                     const float* wt_h, const int* ptr_w, const int* out_w, const float* wt_w, int kw, double scale_w,
+                     void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Denoiser convolutions (deepinv/models/drunet.py:200-210,323-433; dncnn.py:116-131)
  * ------------------------------------------------------------------------------------------

@@ -8,7 +8,7 @@
 # usage: tools/sanitize_emul.sh [memcheck|racecheck] [pytest args...]
 set -u
 MODE=${1:-memcheck}; shift || true
-TESTS=${*:-tests/test_emul_kernels.py tests/test_random_shapes_emul.py tests/test_edge_cases_emul.py tests/test_emul_pipe_kernels.py tests/test_emul_tc32_simt.py tests/test_host_logic_emul.py tests/test_emul_svblur.py tests/test_emul_tv.py tests/test_emul_tgv.py tests/test_emul_spectral_paths.py tests/test_emul_tiledsv.py tests/test_emul_radon_paths.py tests/test_emul_blur_paths.py tests/test_emul_blur3d_paths.py tests/test_emul_mri3d_paths.py tests/test_emul_conv3d.py}
+TESTS=${*:-tests/test_emul_kernels.py tests/test_random_shapes_emul.py tests/test_edge_cases_emul.py tests/test_emul_pipe_kernels.py tests/test_emul_tc32_simt.py tests/test_host_logic_emul.py tests/test_emul_svblur.py tests/test_emul_tv.py tests/test_emul_tgv.py tests/test_emul_spectral_paths.py tests/test_emul_tiledsv.py tests/test_emul_radon_paths.py tests/test_emul_blur_paths.py tests/test_emul_blur3d_paths.py tests/test_emul_mri3d_paths.py tests/test_emul_conv3d.py tests/test_emul_resize.py}
 if [ "$MODE" = "racecheck" ]; then
   rm -f /tmp/dinvk_tsan.*
   DINVK_EMUL_SANITIZE=thread LD_PRELOAD=$(gcc -print-file-name=libtsan.so) \
